@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - headline benchmark of the B200-native LFM sampling path.
+"""bench.py - headline benchmark of the H100-native LFM sampling path.
 
     python bench.py --gpus N --steps K --warmup W            # ours (one process per GPU under torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference algorithm on the host CPU
+    python bench.py ... --dump-outputs DIR    # also write the last timed step's sampled latents to DIR/latents.npy
 
 Workload (BASELINE.json configs[1]): DiT-L/2, 32x32x4 latents, Euler-50 (torchdiffeq-style uniform grid,
 step_size 0.02 => 50 NFE), batch 64 per GPU, synthetic non-degenerate weights (lfm_b200.synthetic
@@ -35,7 +36,7 @@ import torch
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-DEFAULT_GEMM_BN = 512   # lfm_dbg_gemm tile selector of the network's default GEMM kernel (512: 256 x 256 pair tile; 640: 512 x 256)
+DEFAULT_GEMM_BN = 256   # lfm_dbg_gemm tile width of the GEMM kernel (128 x 256 tiles, the network's choice for these shapes)
 MODEL = "DiT-L/2"
 BATCH = 64
 NFE = 50
@@ -50,7 +51,8 @@ def load_peaks():
             d = json.load(f)
         return dict(burst=float(d["bf16_tflops"]), sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                     hbm=float(d["hbm_gbs"]), source="measured (MEASURED_PEAKS.json)")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W board): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s - a ceiling, not a measured rate
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, source="fallback (H100 SXM data sheet, dense BF16)")
 
 
 class ClockSampler:
@@ -127,9 +129,9 @@ def build_unet_celeb512(device, max_batch):
 
 
 def time_dominant_kernel(device, peaks, iters=20):
-    """Roofline of the dominant kernel: the CTA-pair tcgen05 GEMM (gemm2_bf16_tcgen05), on its largest instance
-    in the network (mlp.fc1 + bias + GELU: M = 64*256, N = 4096, K = 1024), timed with CUDA events on the
-    launching stream.  Operands + output = 176 MB > the 126 MB L2."""
+    """Roofline of the dominant kernel: the wgmma GEMM (gemm_bf16_wgmma), on its largest instance in the network
+    (mlp.fc1 + bias + GELU: M = 64*256, N = 4096, K = 1024), timed with CUDA events on the launching stream.
+    Operands + output = 176 MB > the 50 MB L2."""
     from lfm_b200 import _lib
     lib = _lib.load()
     M, N, K = BATCH * 256, 4096, 1024
@@ -140,7 +142,7 @@ def time_dominant_kernel(device, peaks, iters=20):
     s = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
     def run():
-        rc = lib.lfm_dbg_gemm(a.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), None, 0, 256, M, N, K, 1, 512, s)
+        rc = lib.lfm_dbg_gemm(a.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), None, 0, 256, M, N, K, 1, DEFAULT_GEMM_BN, s)
         assert rc == 0, _lib.last_error()
     for _ in range(3):
         run()
@@ -153,14 +155,9 @@ def time_dominant_kernel(device, peaks, iters=20):
     torch.cuda.synchronize(device)
     ms = e0.elapsed_time(e1) / iters
     achieved = 2.0 * M * N * K / (ms * 1e-3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            traffic = json.load(f).get("gemm_fc1_dram_bytes_per_launch")
-    return {"bound": "tensor", "kernel": "gemm2_bf16_tcgen05<EPI_BIAS_GELU_BF16> (cta_group::2, 256x256 tile) M=16384 N=4096 K=1024",
+    return {"bound": "tensor", "kernel": "gemm_bf16_wgmma<256, EPI_BIAS_GELU_BF16> (128x256 tile) M=16384 N=4096 K=1024",
             "achieved": round(achieved, 1), "peak": peaks["burst"], "unit": "TFLOP/s", "frac": round(achieved / peaks["burst"], 4),
-            "traffic": traffic, "us_per_launch": round(ms * 1e3, 2), "peak_source": peaks["source"] + ", burst (kernel timed alone)"}
+            "us_per_launch": round(ms * 1e3, 2), "peak_source": peaks["source"] + ", burst (kernel timed alone)"}
 
 
 def usable_threads():
@@ -208,7 +205,7 @@ def workload_config(world):
     """The `config` object of the GPU arm."""
     return {"workload": f"{MODEL} 32x32x4 latents, Euler-{NFE} (step_size {STEP_SIZE}), batch {BATCH}/GPU, "
                         f"synthetic non-degenerate init (seed {WEIGHT_SEED}), {'dp' + str(world)}",
-            "l2": "inputs larger than L2: 0.9 GB of weights + 0.7 GB of activations stream per NFE (L2 = 126 MB)",
+            "l2": "inputs larger than L2: 0.9 GB of weights + 0.7 GB of activations stream per NFE (L2 = 50 MB)",
             "global_batch": BATCH * world, "nfe_per_image": NFE}
 
 
@@ -268,7 +265,7 @@ FLOPS_UNET_CELEB512 = 189.72e9
 
 
 def gemm_vs_cublas(device, iters=20):
-    """The four DiT-L/2 linear layers at batch 64 (M = 16384): our CTA-pair tcgen05 kernel WITH its fused epilogue
+    """The four DiT-L/2 linear layers at batch 64 (M = 16384): our wgmma kernel WITH its fused epilogue
     (bias / GELU / gated residual add) against (a) the bare torch.matmul (cuBLAS) of the same operands - `ratio` - and
     (b) the same OPERATION through the library (cuBLASLt bias epilogue + separate elementwise kernels) -
     `ratio_vs_library_same_op` - on the same box, CUDA events, alternating so that all see the same clocks.  > 1: ours is faster."""
@@ -333,7 +330,7 @@ def gemm_vs_cublas(device, iters=20):
 
 def gpu_eager_baseline(device, nfe_run=10):
     """The reference network in eager PyTorch on THIS GPU (tests/tools/eager_dit.py): the library baseline a user of the
-    reference gets on a B200 - bf16 autocast + F.scaled_dot_product_attention + TF32 on - and the reference's own
+    reference gets on this GPU - bf16 autocast + F.scaled_dot_product_attention + TF32 on - and the reference's own
     setting, fp32 with TF32 off (test_flow_latent.py:103).  Same weights, batch and Euler grid as the headline; a bounded
     sample of nfe_run Euler steps scaled to Euler-50."""
     from tests.tools import eager_dit
@@ -369,12 +366,16 @@ def gpu_eager_baseline(device, nfe_run=10):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5)  # timed sampling passes, >= 1
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip other_configs / gemm_vs_cublas / gpu_eager_baseline / decode")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the sampled latents of the last timed step to DIR/latents.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
     if args.warmup < 3:
@@ -385,7 +386,7 @@ def main():
     from lfm_b200 import dist as ldist
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); the lfm_b200 hot path has no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device (H100); the lfm_b200 hot path has no CPU fallback")
     rank, world, local = ldist.init_from_env("nccl")
     if world != args.gpus and not (world == 1 and args.gpus == 1):
         if rank == 0:
@@ -409,9 +410,12 @@ def main():
             dist.barrier()
         torch.cuda.synchronize(device)
 
+    last = {}
+
     def step_device():
         xf = lfm_b200.sample_from_model(net, z_dev, {}, sargs)[-1]
-        return ldist.all_gather_batch(xf) if world > 1 else xf
+        last["latents"] = ldist.all_gather_batch(xf) if world > 1 else xf
+        return last["latents"]
 
     def step_e2e():
         z = z_host.to(device, non_blocking=True)
@@ -443,6 +447,11 @@ def main():
         sampler.start()
     ms_total, launches = timed(step_device, args.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path receives: the Euler-50 latents of the last timed step, [BATCH * world, 4, 32, 32] (1 MB per 64)
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), last["latents"].float().cpu().numpy())
     for _ in range(2):
         step_e2e()
     ms_e2e, _ = timed(step_e2e, args.steps)

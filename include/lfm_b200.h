@@ -1,4 +1,4 @@
-/* lfm_b200.h - C ABI of liblfm_b200.so: the B200-native latent flow-matching sampling path.
+/* lfm_b200.h - C ABI of liblfm_b200.so: the H100-native latent flow-matching sampling path.
  *
  * Drop-in boundary for the sampling hot path of VinAIResearch/LFM.  The reference has no native code and
  * therefore no FFI of its own; each entry point below replaces a Python call site of the reference (cited as
@@ -188,13 +188,14 @@ int64_t lfm_launch_count(const lfm_ctx* ctx);
 
 /* ---- kernel-level entry points used by the parity tests (tests/test_gpu_parity.py) ------------------- */
 /* C = A[M,K] W[N,K]^T with epilogue `epi` (0 bias->bf16, 1 bias+gelu->bf16, 2 gated residual fp32, 3 bias->fp32).
- * a, w: bf16 device pointers.  block_n: 128 / 256 (one CTA per tile) or 512 (CTA-pair kernel, 256 x 256 tile). */
+ * a, w: bf16 device pointers.  block_n: tile width 128 or 256 (128 x block_n tiles); 0, 512, 640 or 1024: the width the network
+ * would pick for this shape (the three larger values name tile shapes of earlier builds and are still accepted). */
 int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
                  int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream);
-/* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer -> out [B*256, D] bf16.  variant: 3 = persistent single-TMEM-read kernel (default), 2 = persistent two-pass, 0 = P in TMEM,
- * 1 = P through shared memory.  dbg_s (optional) receives the raw S = q k^T as fp32 [B, H, 256, 256]. */
+/* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer in the timm feature order ({q,k,v} * D + head * 64 + c) -> out [B*256, D]
+ * bf16.  variant 0: the TMA + wgmma kernel the network runs for 256 tokens; 1: the mma.sync flash kernel.  dbg_s must be NULL. */
 int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s, void* stream);
-/* The mma.sync attention kernels of the DiT geometries the tcgen05 kernel does not cover (16 / 64 tokens: whole sequence in registers;
+/* The mma.sync attention kernels of the DiT geometries (16 / 64 tokens: whole sequence in registers;
  * other multiples of 64, e.g. 256 / 1024: keys streamed in chunks of 64).  qkv [B*T, 3*H*ch] bf16 with HEAD-MAJOR features
  * (head * 3 ch + {q,k,v} * ch + c), ch = 64 or 80 (head_dim 72 zero-padded), scale head_dim^-1/2 -> out [B*T, H*ch] bf16. */
 int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream);

@@ -1,9 +1,9 @@
-"""lfm_b200 - B200-native (sm_100a) latent flow-matching sampler: the sampling hot path of VinAIResearch/LFM.
+"""lfm_b200 - H100-native (sm_90a) latent flow-matching sampler: the sampling hot path of VinAIResearch/LFM.
 
 Host-side mirror of the reference's interface for this path; the compute lives in liblfm_b200.so
-(hand-written CUDA: tcgen05 GEMM / attention, TMA, CUDA-graph solver loop) behind the C ABI in
+(hand-written CUDA: wgmma GEMM, mma.sync attention, TMA, CUDA-graph solver loop) behind the C ABI in
 include/lfm_b200.h.  Importing this package never touches the GPU; calling into it without the built library
-or without a B200 raises - there is no CPU or eager-PyTorch fallback.
+or without an H100 raises - there is no CPU or eager-PyTorch fallback.
 """
 from .network import DiT, DiT_models, create_network, get_flow_model  # noqa: F401
 from .unet import UNetModel  # noqa: F401

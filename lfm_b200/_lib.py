@@ -74,7 +74,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is missing: build it with `python -m lfm_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python -m lfm_b200.build` (nvcc, sm_90a). "
             "lfm_b200 has no CPU / eager fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():

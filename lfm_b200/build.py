@@ -1,8 +1,8 @@
-"""Build liblfm_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build liblfm_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m lfm_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so is a build product (git-ignored): build() of __graft_entry__.py or this module makes it.
 """
 import os
 import shutil
@@ -33,7 +33,7 @@ def needs_build():
 def build(force=False, verbose=False):
     if not force and not needs_build():
         return OUT
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-shared", "-Xcompiler", "-fPIC", "-o", OUT, SRC]
     if verbose:
         cmd.insert(-3, "-Xptxas")

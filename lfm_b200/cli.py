@@ -93,7 +93,7 @@ def build_parser():
     p.add_argument("--synthetic_init", type=int, default=None, metavar="SEED", help="seeded weights instead of a checkpoint")
     p.add_argument("--no_decode", action="store_true", help="skip the VAE decode; save latents (.npy)")
     p.add_argument("--vae", type=str, default="native", choices=["native", "diffusers"],
-                   help="native: lfm_b200.AutoencoderKL (sm_100a kernels); diffusers: the reference's torch module")
+                   help="native: lfm_b200.AutoencoderKL (sm_90a kernels); diffusers: the reference's torch module")
     p.add_argument("--synthetic_vae", type=int, default=None, metavar="SEED", help="seeded decoder weights instead of a checkpoint")
     p.add_argument("--writer_threads", type=int, default=8, help="JPEG encoder threads of the --compute_fid loop")
     p.add_argument("--inception_weights", type=str, default=None, metavar="FILE",

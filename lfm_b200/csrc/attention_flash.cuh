@@ -1,15 +1,16 @@
-// lfm_b200 - flash-style attention on warp-level mma.sync for the DiT configurations the tcgen05 kernel (T = 256, head_dim = 64:
-// attention3.cuh) and the whole-sequence-in-registers kernel (T = 16 / 64: attention_mma_kernel, unet.cuh) do not cover:
-//   * 1024-token grids (64 x 64 latents with patch 2: 512-pixel images on a DiT-*/2),
-//   * head_dim 72 (the DiT-XL entries of models/DiT.py:355-365) at 256 tokens - stored padded to CH = 80 channels per head with
-//     zero weight rows, so q.k and P.V are unchanged and the padded output columns are zero.
+// lfm_b200 - flash-style attention on warp-level mma.sync for every DiT configuration and the long-grid UNet attention layers
+// whose sequence does not fit in registers (T = 16 / 64: attention_mma_kernel, unet.cuh):
+//   * 256 tokens with head_dim 64 (every released preset: /2 nets on 32 x 32 latents) and 1024-token grids (64 x 64 latents with
+//     patch 2: 512-pixel images on a DiT-*/2),
+//   * head_dim 72 (the DiT-XL entries of models/DiT.py:355-365) - stored padded to CH = 80 channels per head with zero weight rows,
+//     so q.k and P.V are unchanged and the padded output columns are zero.
 // softmax(q k^T * head_dim^-1/2) v of timm's Attention (models/DiT.py:120; SURVEY D6), keys streamed in chunks of 64 through a
 // double-buffered shared-memory ring (cp.async) with the running-maximum rescaling of FlashAttention-2: one block = 64 query rows of
 // one (sample, head), 4 warps x 16 rows; S = Q K_j^T (m16n8k16 bf16, fp32 accumulate) never leaves registers, the row maximum and
 // the exponentials are fp32, P is rounded to bf16 as the A operand of P V_j.  Same fragment / ldmatrix index patterns as
-// attention_mma_kernel.  qkv rows are head-major: feature = head * 3 CH + {q,k,v} * CH + c (re-ordered once at lfm_set_param).
-// These are not preset configurations of the reference (every released checkpoint is a /2 net on 32 x 32 latents with head_dim 64),
-// so the kernel is sized for correctness and decent speed, not for the tcgen05 roofline.
+// attention_mma_kernel.  Two qkv row layouts (row = 3 C features of one token):
+//   head-major  feature = head * 3 CH + {q,k,v} * CH + c     (head_stride = 3 CH, part_stride = CH; re-ordered once at lfm_set_param)
+//   timm        feature = {q,k,v} * C + head * CH + c        (head_stride = CH,   part_stride = C: the checkpoint's own order)
 #pragma once
 #include "common.cuh"
 // (ldmatrix / mma.sync / cp.async helpers: unet.cuh, included before this file by lfm_api.cu)
@@ -25,7 +26,7 @@ LFM_DEVICE void cp_async_wait_group() {
 template <int CH>
 __global__ void __launch_bounds__(128)
 attention_flash_mma_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int T, int C /* heads * CH */,
-                           int heads, float scale_log2e /* true head_dim^-1/2 * log2(e) */) {
+                           int heads, float scale_log2e /* true head_dim^-1/2 * log2(e) */, int head_stride, int part_stride) {
     pdl_wait();
     pdl_trigger();
     static_assert(CH % 16 == 0, "head channels (padded) must be a multiple of 16");
@@ -40,11 +41,11 @@ attention_flash_mma_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16*
     const int q0 = blockIdx.x * KT;
     const int b = blockIdx.y / heads, h = blockIdx.y % heads;
     const size_t ld = static_cast<size_t>(3) * C;
-    const __nv_bfloat16* base = qkv + static_cast<size_t>(b) * T * ld + static_cast<size_t>(h) * 3 * CH;
+    const __nv_bfloat16* base = qkv + static_cast<size_t>(b) * T * ld + static_cast<size_t>(h) * head_stride;
     auto load_tile = [&](__nv_bfloat16* dst, int which, int row0) {  // 64 rows x CH channels of q / k / v starting at token row0
         for (int i = threadIdx.x; i < KT * CPR; i += 128) {
             const int t = i / CPR, c8 = i % CPR;
-            cp_async_16(dst + t * LD + c8 * 8, base + static_cast<size_t>(row0 + t) * ld + which * CH + c8 * 8);
+            cp_async_16(dst + t * LD + c8 * 8, base + static_cast<size_t>(row0 + t) * ld + which * part_stride + c8 * 8);
         }
     };
     const int nchunks = T / KT;

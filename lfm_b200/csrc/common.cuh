@@ -1,6 +1,6 @@
-// lfm_b200 - sm_100a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// lfm_b200 - sm_90a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), L2 policies, programmatic dependent launch.
 // Hand-written inline PTX; no CUTLASS dependency.  Compile only with
-//   -gencode arch=compute_100a,code=sm_100a
+//   -gencode arch=compute_90a,code=sm_90a
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -106,112 +106,6 @@ constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
-
-template <uint32_t kCols>
-LFM_DEVICE void tmem_alloc(uint32_t* smem_result) {
-    static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "power of two >= 32");
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-LFM_DEVICE void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-LFM_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-LFM_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05: descriptors
-
-// Instruction descriptor, kind::f16, A/B = bf16, D = fp32 (bit layout: cute/arch/mma_sm100_desc.hpp
-// InstrDescriptor: c_format[4,6) a_format[7,10) b_format[10,13) a_major[15] b_major[16] n>>3 [17,23) m>>4 [24,29)).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-           ((M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type = 2 at bits [61,64)), version 1 at [46,48).
-//   K-major operand  (rows of 64 bf16 = 128 B, 8-row atoms of 1024 B):  LBO = 16 B (ignored), SBO = 1024 B.
-//   MN-major operand (64 MN elements contiguous = 128 B per K index, 8 K indices per 1024 B atom):
-//     LBO = byte distance between 64-element MN groups, SBO = 1024 B (next 8 K indices).
-LFM_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= 1ull << 46;
-    d |= 2ull << 61;
-    return d;
-}
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05: MMA issue / commit
-
-// D[tmem] (+)= A[smem] * B[smem]
-LFM_DEVICE void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-LFM_DEVICE void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-LFM_DEVICE void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM <-> registers.  32x32b: thread i of warp w touches TMEM lane 32*(w%4)+i, N consecutive columns.
-
-LFM_DEVICE void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-LFM_DEVICE void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-LFM_DEVICE void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-LFM_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-LFM_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------
 // small math helpers
 
 LFM_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
@@ -231,67 +125,10 @@ LFM_DEVICE float gelu_tanh(float x) {
     const float hx = 0.5f * x;
     return fmaf(hx, tanh_fast(inner), hx);
 }
-// GELU(tanh) of two values at once with Blackwell's packed fp32 arithmetic (fma / mul .f32x2: one issue slot per PAIR):
-// 5 packed operations + 2 MUFU.TANH instead of 10 scalar operations + 2 MUFU.  Same formula, same fp32 precision.
-LFM_DEVICE void gelu_tanh_x2(float& a, float& b) {
-    const float k0 = 0.7978845608028654f, k0k1 = 0.7978845608028654f * 0.044715f;
-    uint64_t x, x2, ic, in, hx, o, K0, K0K1, HALF;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(x) : "f"(a), "f"(b));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(K0) : "f"(k0));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(K0K1) : "f"(k0k1));
-    asm("mov.b64 %0, {%1, %1};" : "=l"(HALF) : "f"(0.5f));
-    asm("mul.rn.f32x2 %0, %1, %1;" : "=l"(x2) : "l"(x));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(ic) : "l"(K0K1), "l"(x2), "l"(K0));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(in) : "l"(x), "l"(ic));
-    float i0, i1;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(i0), "=f"(i1) : "l"(in));
-    const float t0 = tanh_fast(i0), t1 = tanh_fast(i1);
-    uint64_t t;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(t) : "f"(t0), "f"(t1));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(hx) : "l"(x), "l"(HALF));
-    asm("fma.rn.f32x2 %0, %1, %2, %1;" : "=l"(o) : "l"(hx), "l"(t));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(o));
-}
-LFM_DEVICE void add_x2(float& a, float& b, float c, float d) {  // (a, b) += (c, d) in one packed instruction
-    uint64_t x, y;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(x) : "f"(a), "f"(b));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(y) : "f"(c), "f"(d));
-    asm("add.rn.f32x2 %0, %0, %1;" : "+l"(x) : "l"(y));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(x));
-}
-LFM_DEVICE void mul_x2(float& a, float& b, float c, float d) {  // (a, b) *= (c, d)
-    uint64_t x, y;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(x) : "f"(a), "f"(b));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(y) : "f"(c), "f"(d));
-    asm("mul.rn.f32x2 %0, %0, %1;" : "+l"(x) : "l"(y));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(x));
-}
-// packed-pair building blocks (one issue slot per pair of fp32 values)
-LFM_DEVICE uint64_t pk2(float a, float b) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-LFM_DEVICE void upk2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-LFM_DEVICE uint64_t add2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-LFM_DEVICE uint64_t mul2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-LFM_DEVICE uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
 LFM_DEVICE float silu(float x) { return x / (1.0f + __expf(-x)); }
 // x * rcp.approx(1 + ex2.approx(..)): 5 instructions, 2 of them MUFU, relative error ~2 ulp of fp32 (the result is rounded to bf16).
 // The IEEE division above compiles to MUFU.RCP + Newton steps + FCHK + a slow-path call per element, which made the GroupNorm
-// apply pass issue-bound at ~60 instructions per element (2.4 TB/s instead of the HBM rate).
+// apply pass issue-bound at ~60 instructions per element instead of bound by its bytes.
 LFM_DEVICE float silu_fast(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 
 LFM_DEVICE float warp_sum(float v) {
@@ -305,9 +142,7 @@ LFM_DEVICE float warp_max(float v) {
     return v;
 }
 
-// L2 eviction-priority policies for bulk-async (TMA) traffic.  The fp32 residual stream (67 MB at batch 64) is re-read by
-// every LayerNorm and read-modify-written by every residual GEMM: marked evict_last it stays resident in the 126 MB L2
-// while the larger activations (qkv, MLP hidden) stream through with normal priority.
+// L2 eviction-priority policies for bulk-async (TMA) traffic (the LayerNorm pass's loads of the residual stream with LFM_L2_HINT).
 LFM_DEVICE uint64_t l2_policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));

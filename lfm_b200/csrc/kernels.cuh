@@ -1,6 +1,6 @@
 // lfm_b200 - the non-GEMM kernels of the DiT velocity network and the ODE-solver arithmetic.
 // All HBM- or latency-bound; plain CUDA cores, vectorised, coalesced.  fp32 everywhere except the bf16 tensors
-// that feed the tcgen05 GEMMs.
+// that feed the wgmma GEMMs.
 #pragma once
 #include "common.cuh"
 
@@ -133,8 +133,8 @@ patch_embed_kernel(const float* __restrict__ x, int x_rows, const float* __restr
 // stage, so loads of later rows are always in flight while the 8 warps normalise the current ones.
 // One warp per row, two-pass statistics in registers, coalesced bf16 stores.
 // 16 warps, one row each per stage: the per-row chain (shared-memory reads -> two warp reductions -> rsqrt -> modulate -> store, ~1500
-// clk with its waits) is latency-bound, and with 8 warps the kernel took 19 us whether x came from HBM or from L2
-// (tests/tools/l2_residency.cu: 21.4 us after plain stores, 24.6 us after a flush, event-timed).
+// clk with its waits) is latency-bound, so more rows in flight per SM hide more of it (tests/tools/l2_residency.cu times the pass with x
+// in L2 and after a flush).
 // Two shapes are kept for A/B runs (LFM_LN_ROWS = 8 | 16): 8 rows x 4 stages with per-warp modulation loads (round 1), and 16 rows x 3
 // stages with the tile's shift / scale vectors staged next to its rows.
 __host__ __device__ constexpr int ln_stages(int NV, int ROWS) { return ROWS == 8 ? 4 : (NV > 8 ? 2 : 3); }  // 16 rows: 3 x 72 KB at D = 1024
@@ -153,11 +153,7 @@ LFM_DEVICE void bulk_load_1d_hint(void* smem_dst, const void* gsrc, uint32_t byt
                  : "memory");
 }
 
-// X2 (LFM_LN_X2, 16-row shape): the row arithmetic in Blackwell's packed f32x2 instructions - the pass is bound by the length of each
-// warp's dependent instruction chain (407 warp instructions per row at ~37 % issue utilisation, profiles/r2y), and two thirds of
-// those are fp32 adds / multiplies / fmas that pair up: sum 32 -> 16, variance 64 -> 32, modulate 128 -> 64 issue slots per row.
-// y = (x - mean) * (rstd * (1 + scale)) + shift: the same value up to one rounding of the product.
-template <int NV, int kLnRows, bool X2 = false>  // NV = D / 128 float4 per lane; kLnRows = rows per stage = warps per block
+template <int NV, int kLnRows>  // NV = D / 128 float4 per lane; kLnRows = rows per stage = warps per block
 __global__ void __launch_bounds__(kLnRows * 32, 1)
 ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, const float* __restrict__ shift,
                    const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int order_flags) {
@@ -166,9 +162,8 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
     const int order = order_flags & 3;          // tile order (below)
     const bool keep = (order_flags & 4) != 0;   // x is the residual stream: load with the evict_last L2 policy
     const uint64_t policy = keep ? l2_policy_evict_last() : 0;
-    // a stage = kLnRows rows of x + the shift and scale vectors of the tile's sample.  (Every warp used to fetch its own copy of
-    // the two vectors from L2 - 8 KB per 4 KB row, 134 MB per launch on top of the 67 MB of x: the pass was bound by L2 -> SM
-    // bandwidth at 19 us whether x sat in L2 or in HBM; tests/tools/l2_residency.cu.)
+    // a stage = kLnRows rows of x + the shift and scale vectors of the tile's sample: one copy of the two vectors per tile instead of
+    // one per warp (8 KB per 4 KB row, twice the bytes of x through L2 -> SM).
     constexpr uint32_t kStageBytes = (kLnRows + (kLnRows == 16 ? 2 : 0)) * D * 4;
     const bool mod_smem = kLnRows == 16 && rows_per_sample % kLnRows == 0;  // a tile never straddles two samples
     extern __shared__ __align__(128) uint8_t ln_smem[];
@@ -234,55 +229,6 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
             }
         }
         mbar_wait(&full_bar[stage], parity);
-        if constexpr (X2) {
-            if (ok) {
-                const float4* xp = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + warp * D * 4);
-                uint64_t pr[NV][2];
-                uint64_t acc = pk2(0.f, 0.f);
-#pragma unroll
-                for (int m = 0; m < NV; ++m) {
-                    const float4 t4 = xp[m * 32 + lane];
-                    pr[m][0] = pk2(t4.x, t4.y);
-                    pr[m][1] = pk2(t4.z, t4.w);
-                    acc = add2(acc, add2(pr[m][0], pr[m][1]));
-                }
-                float ax, ay;
-                upk2(acc, ax, ay);
-                const float mean = warp_sum(ax + ay) / static_cast<float>(D);
-                const uint64_t nmean = pk2(-mean, -mean);
-                uint64_t q0 = pk2(0.f, 0.f), q1 = pk2(0.f, 0.f);
-#pragma unroll
-                for (int m = 0; m < NV; ++m) {
-                    const uint64_t d0 = add2(pr[m][0], nmean), d1 = add2(pr[m][1], nmean);
-                    q0 = fma2(d0, d0, q0);
-                    q1 = fma2(d1, d1, q1);
-                }
-                float qx, qy;
-                upk2(add2(q0, q1), qx, qy);
-                const float rstd = rsqrtf(warp_sum(qx + qy) / static_cast<float>(D) + 1e-6f);
-                const uint64_t r2 = pk2(rstd, rstd), one2 = pk2(1.f, 1.f);
-                uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
-                const float4* shs = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + kLnRows * D * 4);
-                const size_t boff = static_cast<size_t>(row / rows_per_sample) * mod_stride;
-                const float4* shg = reinterpret_cast<const float4*>(shift + boff);
-                const float4* scg = reinterpret_cast<const float4*>(scale + boff);
-#pragma unroll
-                for (int m = 0; m < NV; ++m) {
-                    const float4 sh = mod_smem ? shs[m * 32 + lane] : __ldg(shg + m * 32 + lane);
-                    const float4 sc = mod_smem ? shs[D / 4 + m * 32 + lane] : __ldg(scg + m * 32 + lane);
-                    const uint64_t g0 = mul2(add2(pk2(sc.x, sc.y), one2), r2), g1 = mul2(add2(pk2(sc.z, sc.w), one2), r2);
-                    const uint64_t o0 = fma2(add2(pr[m][0], nmean), g0, pk2(sh.x, sh.y));
-                    const uint64_t o1 = fma2(add2(pr[m][1], nmean), g1, pk2(sh.z, sh.w));
-                    float a, b, c, d;
-                    upk2(o0, a, b);
-                    upk2(o1, c, d);
-                    yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
-                }
-            }
-            __syncthreads();  // every warp has consumed this stage
-            if (threadIdx.x == 0 && i + kLnStages < my_tiles) issue(i + kLnStages);
-            continue;
-        }
         if (ok) {
             const float4* xp = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + warp * D * 4);
             float4 v[NV];
@@ -329,7 +275,7 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
 // The same pass without the shared-memory ring (LFM_LN_ROWS=0): one row per warp straight from global memory into registers, 64
 // registers so that 32 warps are resident per SM (8 independent row chains per scheduler instead of 4), the grid sweeping M in
 // order (upwards, or downwards for order 2).  Same arithmetic in the same order as ln_modulate_kernel: identical results.
-template <int NV, int THREADS = 256, int MINB = 4, bool X2 = false>
+template <int NV, int THREADS = 256, int MINB = 4>
 __global__ void __launch_bounds__(THREADS, MINB)
 ln_modulate_direct_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, const float* __restrict__ shift,
                           const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int order_flags) {
@@ -348,65 +294,28 @@ ln_modulate_direct_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict
         const float4* shp = reinterpret_cast<const float4*>(shift + boff);
         const float4* scp = reinterpret_cast<const float4*>(scale + boff);
         uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
-        if constexpr (X2) {
-            uint64_t pr[NV][2];
+        float4 v[NV];
 #pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const float4 t4 = xp[m * 32 + lane];
-                pr[m][0] = pk2(t4.x, t4.y);
-                pr[m][1] = pk2(t4.z, t4.w);
-            }
-            uint64_t acc = pk2(0.f, 0.f);
+        for (int m = 0; m < NV; ++m) v[m] = xp[m * 32 + lane];
+        float s = 0.f;
 #pragma unroll
-            for (int m = 0; m < NV; ++m) acc = add2(acc, add2(pr[m][0], pr[m][1]));
-            float ax, ay;
-            upk2(acc, ax, ay);
-            const float mean = warp_sum(ax + ay) / static_cast<float>(D);
-            const uint64_t nmean = pk2(-mean, -mean);
-            uint64_t q0 = pk2(0.f, 0.f), q1 = pk2(0.f, 0.f);
+        for (int m = 0; m < NV; ++m) s += (v[m].x + v[m].y) + (v[m].z + v[m].w);
+        const float mean = warp_sum(s) / static_cast<float>(D);
+        float ss = 0.f;
 #pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const uint64_t d0 = add2(pr[m][0], nmean), d1 = add2(pr[m][1], nmean);
-                q0 = fma2(d0, d0, q0);
-                q1 = fma2(d1, d1, q1);
-            }
-            float qx, qy;
-            upk2(add2(q0, q1), qx, qy);
-            const float rstd = rsqrtf(warp_sum(qx + qy) / static_cast<float>(D) + 1e-6f);
-            const uint64_t r2 = pk2(rstd, rstd), one2 = pk2(1.f, 1.f);
+        for (int m = 0; m < NV; ++m) {
+            const float a = v[m].x - mean, b = v[m].y - mean, c = v[m].z - mean, d = v[m].w - mean;
+            ss += (a * a + b * b) + (c * c + d * d);
+        }
+        const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(D) + 1e-6f);
 #pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const float4 sh = __ldg(shp + m * 32 + lane), sc = __ldg(scp + m * 32 + lane);
-                const uint64_t g0 = mul2(add2(pk2(sc.x, sc.y), one2), r2), g1 = mul2(add2(pk2(sc.z, sc.w), one2), r2);
-                float a, b, c, d;
-                upk2(fma2(add2(pr[m][0], nmean), g0, pk2(sh.x, sh.y)), a, b);
-                upk2(fma2(add2(pr[m][1], nmean), g1, pk2(sh.z, sh.w)), c, d);
-                yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
-            }
-        } else {
-            float4 v[NV];
-#pragma unroll
-            for (int m = 0; m < NV; ++m) v[m] = xp[m * 32 + lane];
-            float s = 0.f;
-#pragma unroll
-            for (int m = 0; m < NV; ++m) s += (v[m].x + v[m].y) + (v[m].z + v[m].w);
-            const float mean = warp_sum(s) / static_cast<float>(D);
-            float ss = 0.f;
-#pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const float a = v[m].x - mean, b = v[m].y - mean, c = v[m].z - mean, d = v[m].w - mean;
-                ss += (a * a + b * b) + (c * c + d * d);
-            }
-            const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(D) + 1e-6f);
-#pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const float4 sh = __ldg(shp + m * 32 + lane), sc = __ldg(scp + m * 32 + lane);
-                const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
-                const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
-                const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
-                const float d = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
-                yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
-            }
+        for (int m = 0; m < NV; ++m) {
+            const float4 sh = __ldg(shp + m * 32 + lane), sc = __ldg(scp + m * 32 + lane);
+            const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
+            const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
+            const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
+            const float d = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
+            yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
         }
     }
 }

@@ -1,5 +1,5 @@
 // lfm_b200 - C ABI (include/lfm_b200.h): context, parameter upload, DiT forward, ODE solvers.
-// Single translation unit; build:  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared ...
+// Single translation unit; build:  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared ...
 #include "../../include/lfm_b200.h"
 
 #include <algorithm>
@@ -13,14 +13,9 @@
 #include <unordered_map>
 #include <vector>
 
-#include "attention.cuh"
-#include "attention2.cuh"
-#include "attention3.cuh"
 #include "common.cuh"
 #include "gemm.cuh"
-#include "gemm2.cuh"
-#include "gemm4.cuh"
-#include "gemm5.cuh"
+#include "attention_wgmma.cuh"
 #include "kernels.cuh"
 #include "unet.cuh"
 #include "attention_flash.cuh"
@@ -73,21 +68,6 @@ static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint
     CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-// Output tile map for the TMA-store epilogue: row-major [rows, cols] (bf16 or fp32), box = 128 bytes x 32 rows.
-static bool make_tmap_out(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, bool is_f32) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (fn == nullptr) return false;
-    const uint64_t esz = is_f32 ? 4 : 2;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * esz};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / esz), 32};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(m, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                    const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
 
@@ -149,174 +129,40 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, unsigned block, s
 
 template <int BN, int EPI>
 static cudaError_t launch_gemm_inst(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K,
-                                    const GemmEpi& ep) {
+                                    const GemmEpi& ep, const ConvGeom& cg, int ksplit, int split_row_pitch) {
     static DevOnce once;
-    auto kern = gemm_bf16_tcgen05<BN, EPI>;
+    auto kern = gemm_bf16_wgmma<BN, EPI>;
     if (cudaError_t e = smem_opt_in(once, kern, GemmCfg<BN>::kSmemBytes)) return e;
-    const int tiles = ((M + kGemmBlockM - 1) / kGemmBlockM) * ((N + BN - 1) / BN);
-    const int grid = tiles < g_num_sms ? tiles : g_num_sms;
-    return launch_k(kern, dim3(grid), kGemmThreads, GemmCfg<BN>::kSmemBytes, s, ta, tb, M, N, K, ep);
+    const int items = ((M + kGemmBlockM - 1) / kGemmBlockM) * ((N + BN - 1) / BN) * ksplit;
+    const int grid = items < g_num_sms ? items : g_num_sms;
+    return launch_k(kern, dim3(grid), kGemmThreads, GemmCfg<BN>::kSmemBytes, s, ta, tb, M, N, K, ep, cg, ksplit, split_row_pitch);
 }
 
-// 2-CTA pair kernel (256 x 256 tile per cluster of two CTAs)
-template <int EPI>
-static cudaError_t launch_gemm2_inst(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb,
-                                     const CUtensorMap& tout, int M, int N, int K, const GemmEpi& ep,
-                                     ConvGeom cg = ConvGeom{0, 0, 0, 0, 1}, const CUtensorMap* tbh = nullptr, int ksplit = 1,
-                                     int split_row_pitch = 0, bool starved_halves = false) {
+// softmax(q k^T / 8) v for 256 tokens, head_dim 64, timm qkv order (attention_wgmma.cuh); tqkv: box {64, kGemmBoxRows} over [rows, 3 C]
+static cudaError_t launch_attention_wgmma(cudaStream_t s, const CUtensorMap& tqkv, __nv_bfloat16* out, int C, int heads, int samples) {
     static DevOnce once;
-    auto kern = gemm2_bf16_tcgen05<EPI>;
-    if (cudaError_t e = smem_opt_in(once, kern, kG2SmemBytes)) return e;
-    const int tiles = ((M + 255) / 256) * ((N + kG2BlockN - 1) / kG2BlockN) * ksplit;
-    int clusters = g_num_sms / 2;
-    static const int split_env = env_int("LFM_GEMM_SPLIT", 1);
-    const bool can_split = tbh != nullptr && split_env != 0;
-    static const int halves_env = env_int("LFM_GEMM_HALVES", 1);  // A/B switch of the tile-starved mode below
-    // Tile-starved launches (2 x tiles <= CTA pairs; small sampling batches) run entirely in 256 x 128 half tiles (allow_split = 2).
-    // Measured limit of the rule (r3j): extending it to every launch of at most one wave (tiles <= CTA pairs, e.g. the 64 tiles of the
-    // residual GEMMs at 4096 token rows) is SLOWER, 3.66 vs 3.29 ms per evaluation at batch 16 - an N = 128 MMA moves the same A
-    // operand through shared memory as an N = 256 one, so two half tiles cost more than one tile and the hidden epilogue does not pay for it.
-    int allow = can_split ? 1 : 0;
-    if (starved_halves && halves_env && can_split && ksplit == 1 && 2 * tiles <= clusters) {
-        allow = 2;
-        clusters = 2 * tiles;
-    } else if (tiles < clusters) {
-        clusters = tiles;
-    }
-    return launch_k(kern, dim3(2 * clusters), kG2Threads, kG2SmemBytes, s, ta, tb, tout, tbh != nullptr ? *tbh : tb, M, N, K, ep, cg,
-                    allow, ksplit, split_row_pitch);
+    if (cudaError_t e = smem_opt_in(once, attention_wgmma_t256_d64, kAttnSmemBytes)) return e;
+    const int items = samples * heads * 2;
+    const int grid = items < g_num_sms ? items : g_num_sms;
+    return launch_k(attention_wgmma_t256_d64, dim3(grid), kAttnThreads, kAttnSmemBytes, s, tqkv, out, C, heads, items,
+                    0.125f * 1.4426950408889634f);
 }
 
-// Pair kernel with the LayerNorm finisher (ep.ln_out != nullptr; N == D): see GemmEpi::rb_count
-static cudaError_t launch_gemm2_fin(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, int M,
-                                    int N, int K, const GemmEpi& ep, const CUtensorMap* tbh) {
-    static DevOnce once;
-    auto kern = gemm2_bf16_tcgen05<EPI_GATE_RESID_F32, true>;
-    if (cudaError_t e = smem_opt_in(once, kern, kG2SmemBytes)) return e;
-    const int tiles = ((M + 255) / 256) * ((N + kG2BlockN - 1) / kG2BlockN);
-    int clusters = g_num_sms / 2;
-    if (tiles < clusters) clusters = tiles;
-    static const int split_env = env_int("LFM_GEMM_SPLIT", 1);
-    const ConvGeom cg{0, 0, 0, 0, 1};
-    return launch_k(kern, dim3(2 * clusters), kG2ThreadsFin, kG2SmemBytes, s, ta, tb, tout, tbh != nullptr ? *tbh : tb, M, N, K, ep, cg,
-                    (tbh != nullptr && split_env) ? 1 : 0, 1, 0);
+// Tile width: 256 columns, unless N fits in 128 or the 256-wide tiles would leave more than half of the SMs idle (small
+// sampling batches) - then 128, which doubles the tiles of the launch.
+static int pick_block_n(int M, int N) {
+    const int tiles256 = ((M + kGemmBlockM - 1) / kGemmBlockM) * ((N + 255) / 256);
+    return (N <= 128 || 2 * tiles256 <= g_num_sms) ? 128 : 256;
 }
 
-// Pair kernel with the 512 x 256 cluster tile (gemm5.cuh)
-static G5Sched g5_schedule_host(int M, int N, int clusters) {
-    G5Sched s;
-    s.n_blocks = (N + 255) / 256;
-    s.m512 = (M + 511) / 512;
-    const int tiles = s.m512 * s.n_blocks;
-    s.full_count = (tiles / clusters) * clusters;
-    const int rem = tiles - s.full_count;
-    s.split = 1;
-    if (rem > 0) {
-        int best_num = (rem + clusters - 1) / clusters * 4, best = 1;
-        for (int f = 2; f <= 4; f *= 2) {
-            const int c = ((rem * f + clusters - 1) / clusters) * (4 / f);
-            if (c < best_num) {
-                best_num = c;
-                best = f;
-            }
-        }
-        s.split = best;
-    }
-    s.num_items = s.full_count + rem * s.split;
-    return s;
-}
-template <int EPI>
-static cudaError_t launch_gemm5_inst(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
-                                     const CUtensorMap& tbh, int M, int N, int K, const GemmEpi& ep,
-                                     ConvGeom cg = ConvGeom{0, 0, 0, 0, 1}) {
-    static DevOnce once;
-    auto kern = gemm5_bf16_tcgen05<EPI>;
-    if (cudaError_t e = smem_opt_in(once, kern, kG5SmemBytes)) return e;
-    const int sched_clusters = g_num_sms / 2;
-    const G5Sched sc = g5_schedule_host(M, N, sched_clusters);
-    const int clusters = sc.num_items < sched_clusters ? sc.num_items : sched_clusters;
-    static const int skew = std::min(std::max(env_int("LFM_G5_SKEW", kG5Skew), 0), kG5Skew);
-    static const int dbg = env_int("LFM_G5_DBG", 0);
-    return launch_k(kern, dim3(2 * clusters), kG5Threads, kG5SmemBytes, s, ta, tb, tout, tbh, M, N, K, ep, cg, sched_clusters, skew, dbg);
-}
-
-// 4-CTA cluster kernel (two pairs sharing A by multicast; 256 x 512 block per cluster)
-template <int EPI>
-static cudaError_t launch_gemm4_inst(cudaStream_t s, const CUtensorMap& ta64, const CUtensorMap& tb, const CUtensorMap& tout,
-                                     int M, int N, int K, const GemmEpi& ep) {
-    static int max_clusters_dev[64];  // per device; 0 = not queried yet
-    static DevOnce once;
-    auto kern = gemm4_bf16_tcgen05<EPI>;
-    int dev = 0;
-    if (cudaError_t e = cudaGetDevice(&dev)) return e;
-    int& max_clusters = max_clusters_dev[dev & 63];
-    if (max_clusters <= 0) {
-        cudaError_t e = smem_opt_in(once, kern, kG4SmemBytes);
-        if (e != cudaSuccess) return e;
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(4 * (g_num_sms / 4));
-        cfg.blockDim = dim3(kG4Threads);
-        cfg.dynamicSmemBytes = kG4SmemBytes;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = 4;
-        at[0].val.clusterDim.y = 1;
-        at[0].val.clusterDim.z = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = 1;
-        int nc = 0;
-        e = cudaOccupancyMaxActiveClusters(&nc, kern, &cfg);
-        if (e != cudaSuccess) return e;
-        max_clusters = nc > 0 ? nc : 1;
-        if (env_int("LFM_GEMM4_CLUSTERS", 0) > 0) max_clusters = env_int("LFM_GEMM4_CLUSTERS", 0);
-    }
-    const int n_blocks = (N + kG2BlockN - 1) / kG2BlockN;
-    const int items = ((M + 255) / 256) * ((n_blocks + 1) / 2);
-    const int clusters = items < max_clusters ? items : max_clusters;
-    kern<<<4 * clusters, kG4Threads, kG4SmemBytes, s>>>(ta64, tb, tout, M, N, K, ep);
-    return cudaGetLastError();
-}
-
-// block_n: 128 / 256 = one CTA per 128 x block_n tile; kGemmPair (512) = CTA pair per 256 x 256 tile;
-// kGemmQuad (1024) = cluster of two pairs per 256 x 512 block (A multicast)
-constexpr int kGemmPair = 512;
-constexpr int kGemmQuad = 1024;
-constexpr int kGemmPair512 = 640;  // CTA pair per 512 x 256 tile (gemm5.cuh)
-static inline uint32_t weight_box_rows(int block_n) {
-    return (block_n == kGemmPair || block_n == kGemmQuad || block_n == kGemmPair512) ? 128u : static_cast<uint32_t>(block_n);
-}
-
-static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K,
-                               int epi, int block_n, const GemmEpi& ep, const CUtensorMap* tout = nullptr,
-                               const CUtensorMap* tbh = nullptr, const CUtensorMap* ta64 = nullptr) {
-    if (block_n == kGemmQuad) {
-        if (tout == nullptr || ta64 == nullptr) return cudaErrorInvalidValue;
-        if (epi == EPI_BIAS_BF16) return launch_gemm4_inst<EPI_BIAS_BF16>(s, *ta64, tb, *tout, M, N, K, ep);
-        if (epi == EPI_BIAS_GELU_BF16) return launch_gemm4_inst<EPI_BIAS_GELU_BF16>(s, *ta64, tb, *tout, M, N, K, ep);
-        if (epi == EPI_GATE_RESID_F32) return launch_gemm4_inst<EPI_GATE_RESID_F32>(s, *ta64, tb, *tout, M, N, K, ep);
-        if (epi == EPI_BIAS_F32) return launch_gemm4_inst<EPI_BIAS_F32>(s, *ta64, tb, *tout, M, N, K, ep);
-        return cudaErrorInvalidValue;
-    }
-    if (block_n == kGemmPair512) {
-        if (tout == nullptr || tbh == nullptr) return cudaErrorInvalidValue;
-        if (epi == EPI_BIAS_BF16) return launch_gemm5_inst<EPI_BIAS_BF16>(s, ta, tb, *tout, *tbh, M, N, K, ep);
-        if (epi == EPI_BIAS_GELU_BF16) return launch_gemm5_inst<EPI_BIAS_GELU_BF16>(s, ta, tb, *tout, *tbh, M, N, K, ep);
-        if (epi == EPI_GATE_RESID_F32) return launch_gemm5_inst<EPI_GATE_RESID_F32>(s, ta, tb, *tout, *tbh, M, N, K, ep);
-        if (epi == EPI_BIAS_F32) return launch_gemm5_inst<EPI_BIAS_F32>(s, ta, tb, *tout, *tbh, M, N, K, ep);
-        return cudaErrorInvalidValue;
-    }
-    if (block_n == kGemmPair) {
-        if (tout == nullptr) return cudaErrorInvalidValue;
-        const ConvGeom cg{0, 0, 0, 0, 1};
-        if (epi == EPI_BIAS_BF16) return launch_gemm2_inst<EPI_BIAS_BF16>(s, ta, tb, *tout, M, N, K, ep, cg, tbh, 1, 0, true);
-        if (epi == EPI_BIAS_GELU_BF16) return launch_gemm2_inst<EPI_BIAS_GELU_BF16>(s, ta, tb, *tout, M, N, K, ep, cg, tbh, 1, 0, true);
-        if (epi == EPI_GATE_RESID_F32 && ep.fin_ctl != nullptr) return launch_gemm2_fin(s, ta, tb, *tout, M, N, K, ep, tbh);
-        if (epi == EPI_GATE_RESID_F32) return launch_gemm2_inst<EPI_GATE_RESID_F32>(s, ta, tb, *tout, M, N, K, ep, cg, tbh, 1, 0, true);
-        if (epi == EPI_BIAS_F32) return launch_gemm2_inst<EPI_BIAS_F32>(s, ta, tb, *tout, M, N, K, ep, cg, tbh, 1, 0, true);
-        return cudaErrorInvalidValue;
-    }
+// A and W are tensor maps with a box of {64, kGemmBoxRows} (make_tmap_bf16 / make_tmap_act4d); block_n = 128 or 256
+// (0: pick_block_n).  The batched GEMMs of ConvGeom need block_n 256 when N is a multiple of 256 (W rows of one group).
+static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int epi,
+                               int block_n, const GemmEpi& ep, const ConvGeom& cg = ConvGeom{0, 0, 0, 0, 1}, int ksplit = 1,
+                               int split_row_pitch = 0) {
+    if (block_n == 0) block_n = cg.batch_m > 0 ? 256 : pick_block_n(M, N);
 #define LFM_GEMM_CASE(BN, E) \
-    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E>(s, ta, tb, M, N, K, ep);
+    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E>(s, ta, tb, M, N, K, ep, cg, ksplit, split_row_pitch);
     LFM_GEMM_CASE(256, EPI_BIAS_BF16)
     LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
     LFM_GEMM_CASE(256, EPI_GATE_RESID_F32)
@@ -329,23 +175,12 @@ static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUte
     return cudaErrorInvalidValue;
 }
 
-template <bool P_TMEM>
-static cudaError_t launch_attention_inst(cudaStream_t s, const CUtensorMap& tq, const CUtensorMap& tkv,
-                                         __nv_bfloat16* out, int B, int H, int D, float* dbg_s) {
-    static DevOnce once;
-    auto kern = attention_t256_d64<P_TMEM>;
-    if (cudaError_t e = smem_opt_in(once, kern, attn_smem_bytes<P_TMEM>())) return e;
-    const float scale_log2e = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e), head_dim = 64
-    kern<<<dim3(2, H, B), kAttnThreads, attn_smem_bytes<P_TMEM>(), s>>>(tq, tkv, out, D, scale_log2e, dbg_s);
-    return cudaGetLastError();
-}
-
-template <int NV, int ROWS, bool X2 = false>
+template <int NV, int ROWS>
 static cudaError_t launch_ln_inst2(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
                                    int mod_stride, int rows_per_sample, int M, int order) {
     static DevOnce once;
     const int smem = ln_stages(NV, ROWS) * (ROWS + (ROWS == 16 ? 2 : 0)) * NV * 128 * 4;
-    auto kern = ln_modulate_kernel<NV, ROWS, X2>;
+    auto kern = ln_modulate_kernel<NV, ROWS>;
     if (cudaError_t e = smem_opt_in(once, kern, smem)) return e;
     const int tiles = (M + ROWS - 1) / ROWS;
     const int grid = tiles < g_num_sms ? tiles : g_num_sms;
@@ -354,19 +189,15 @@ static cudaError_t launch_ln_inst2(cudaStream_t s, const float* x, __nv_bfloat16
 template <int NV>
 static cudaError_t launch_ln_inst(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
                                   int mod_stride, int rows_per_sample, int M, int order) {
-    static const int rows = env_int("LFM_LN_ROWS", 16);  // same-box A/B (r2w): 116.99 / 116.72 img/s vs 116.33 / 116.34 with 8
-    static const int x2 = env_int("LFM_LN_X2", 1);  // packed f32x2 row arithmetic: 18.9 -> 18.5 us per launch (profiles/r3c; see ln_modulate_kernel)
-    if (rows == 16 && x2) return launch_ln_inst2<NV, 16, true>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
+    static const int rows = env_int("LFM_LN_ROWS", 16);  // 16-row ring by default; 8 / 0 / 32: the other shapes (A/B runs)
     if (rows == 16) return launch_ln_inst2<NV, 16>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
     if (rows == 0) {
         const int blocks = std::min((M + 7) / 8, 4 * g_num_sms);
-        if (x2) return launch_k(ln_modulate_direct_kernel<NV, 256, 4, true>, dim3(blocks), 256, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
         return launch_k(ln_modulate_direct_kernel<NV>, dim3(blocks), 256, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
     }
     if (rows == 32) {  // one persistent 32-warp block per SM, rows straight from global memory
         const int blocks = std::min((M + 31) / 32, g_num_sms);
-        if (x2) return launch_k(ln_modulate_direct_kernel<NV, 1024, 1, true>, dim3(blocks), 1024, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-        return launch_k(ln_modulate_direct_kernel<NV, 1024, 1, false>, dim3(blocks), 1024, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
+        return launch_k(ln_modulate_direct_kernel<NV, 1024, 1>, dim3(blocks), 1024, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
     }
     return launch_ln_inst2<NV, 8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
 }
@@ -380,25 +211,6 @@ static cudaError_t launch_ln(cudaStream_t s, const float* x, __nv_bfloat16* y, c
         case 9: return launch_ln_inst<9>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
         default: return cudaErrorInvalidValue;
     }
-}
-
-static cudaError_t launch_attention2(cudaStream_t s, const CUtensorMap& tkv, const CUtensorMap& tout, int B, int H, int D,
-                                     int variant = 2, int reverse = 0) {
-    static DevOnce once2, once3;
-    if (cudaError_t e = smem_opt_in(once2, attention2_t256_d64, kA2SmemBytes)) return e;
-    static DevOnce once3x;
-    static const int attn_x2 = env_int("LFM_ATTN_X2", 1);  // packed f32x2 softmax arithmetic: 40.4 -> 39.0 us per launch (profiles/r3c)
-    if (cudaError_t e = smem_opt_in(once3, attention3_t256_d64<false>, kA2SmemBytes)) return e;
-    if (cudaError_t e = smem_opt_in(once3x, attention3_t256_d64<true>, kA2SmemBytes)) return e;
-    const float scale_log2e = 0.125f * 1.4426950408889634f;
-    const int items = B * H;
-    const int grid = items < g_num_sms ? items : g_num_sms;
-    if (variant == 3)
-        return launch_k(attn_x2 ? attention3_t256_d64<true> : attention3_t256_d64<false>, dim3(grid), kA2Threads, kA2SmemBytes, s, tkv,
-                        tout, D, H, items, scale_log2e, reverse);
-    else
-        attention2_t256_d64<<<grid, kA2Threads, kA2SmemBytes, s>>>(tkv, tout, D, H, items, scale_log2e);
-    return cudaGetLastError();
 }
 
 static inline unsigned blocks_for(size_t n, int threads = 256) { return static_cast<unsigned>((n + threads - 1) / threads); }
@@ -424,7 +236,6 @@ struct BlockW {
     __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;
     float *b_qkv, *b_proj, *b_fc1, *b_fc2;
     CUtensorMap tm_qkv, tm_proj, tm_fc1, tm_fc2;
-    CUtensorMap tmh_qkv, tmh_proj, tmh_fc1, tmh_fc2;  // box {64, 64}: half-width tail tiles of the pair GEMM
 };
 
 struct UNetState;
@@ -437,19 +248,13 @@ struct lfm_ctx {
     int num_sms = 0;
     int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, Nmod = 0, HW = 0, chw = 0;
     int dh = 64, dhp = 64, Dq = 0;  // head_dim, its stored (zero-padded) width and the width H * dhp of the attention tensors
-    bool qkv_head_major = false;    // qkv rows re-ordered for the mma.sync attention kernels (everything but T = 256 with head_dim 64)
+    bool qkv_head_major = false;    // qkv rows re-ordered head-major (everything but T = 256 with head_dim 64, see lfm_create)
     int max_rows = 0;
     bool finalized = false;
     std::string err;
     int64_t launches = 0;
-    int attn_variant = 0;  // 0 = P in TMEM, 1 = P via smem
     int zigzag = 0;        // LFM_ZIGZAG: alternate the row-sweep direction of consecutive kernels (L2 reuse)
-    int l2_hint = 0;       // LFM_L2_HINT: evict_last L2 policy on the residual stream's TMA traffic (measured: no gain)
-    int ln_fuse = 1;       // LFM_LN_FUSE: LayerNorm + modulate of the next layer produced by the residual GEMM's finisher warps
-    int* rb_count = nullptr;  // per 256-row block arrival counters of the finisher (GemmEpi::rb_count)
-    int* fin_ctl = nullptr;   // two control blocks {ticket, tail, -, -, queue[m_blocks]} of the finisher (GemmEpi::fin_ctl)
-    int fin_stride = 0;
-    int bn_qkv = 256, bn_proj = 256, bn_fc1 = 256, bn_fc2 = 256, bn_mod = 256;
+    int l2_hint = 0;       // LFM_L2_HINT: evict_last L2 policy on the LayerNorm pass's loads of the residual stream
 
     std::unordered_map<std::string, ParamSlot> params;
     std::vector<void*> allocs;
@@ -466,9 +271,8 @@ struct lfm_ctx {
     // workspace
     float *x_tok = nullptr, *mod = nullptr, *tfreq = nullptr, *h1 = nullptr, *v_net = nullptr;
     __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
-    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu, tm_qkv_q, tm_qkv_kv;
-    CUtensorMap tmo_qkv, tmo_hmid, tmo_xtok;  // TMA-store epilogue targets
-    CUtensorMap tm64_xn, tm64_attn, tm64_hmid;  // box {64, 64}: quarter A slabs of the 4-CTA multicast kernel
+    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
+    CUtensorMap tm_qkv_attn;  // qkv as read by the 256-token attention (timm order only)
 
     // solver state
     cudaStream_t stream = nullptr;
@@ -560,7 +364,7 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     if (device < 0 || device >= ndev) return fail(nullptr, "lfm_create: bad device %d", device);
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
-    if (prop.major != 10) return fail(nullptr, "lfm_create: device %d is sm_%d%d; this library is sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9) return fail(nullptr, "lfm_create: device %d is sm_%d%d; this library is sm_90a only", device, prop.major, prop.minor);
     ctx = new lfm_ctx();
     ctx->d = *desc;
     ctx->device = device;
@@ -576,15 +380,13 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->HW = desc->img_resolution;
     ctx->chw = ctx->C * ctx->HW * ctx->HW;
     ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
-    ctx->attn_variant = env_int("LFM_ATTN_VARIANT", 3);
     ctx->zigzag = env_int("LFM_ZIGZAG", 1);
     ctx->l2_hint = env_int("LFM_L2_HINT", 0);
-    ctx->ln_fuse = env_int("LFM_LN_FUSE", 0);  // measured (r2b): the in-kernel LayerNorm finisher is 2.6x SLOWER end to end - off
     const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T;
     const int ps = desc->patch_size;
     const int P = ctx->C * ps * ps;  // elements of one patch = out-features of the final linear
-    // Only 256 tokens with head_dim 64 run on the tcgen05 attention kernel (native timm qkv order).  Everything else - 16 / 64 / 1024
-    // tokens, head_dim 72 (DiT-XL, stored padded to 80) - runs on the mma.sync kernels, which read head-major qkv rows.
+    // 256 tokens with head_dim 64 (every released preset) keep the checkpoint's timm qkv order, which the flash kernel reads directly.
+    // Everything else - 16 / 64 / 1024 tokens, head_dim 72 (DiT-XL, stored padded to 80) - stores the qkv rows head-major.
     ctx->dh = desc->hidden_size / desc->num_heads;
     ctx->dhp = ctx->dh == 72 ? 80 : 64;
     ctx->Dq = desc->num_heads * ctx->dhp;
@@ -720,12 +522,6 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
     return 0;
 }
 
-static int pick_bn(int N, const char* env, int dflt) {
-    int bn = env_int(env, dflt);
-    if (bn != 128 && bn != 256 && bn != kGemmPair && bn != kGemmQuad && bn != kGemmPair512) bn = dflt;
-    return bn;
-}
-
 static int alloc_solver_state(lfm_ctx* ctx, int R) {
     // solver state (sized for R latent rows)
     const size_t nst = (size_t)R * ctx->chw;
@@ -780,46 +576,20 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (dev_alloc(ctx, &ctx->tfreq, (size_t)R * 256)) return 1;
     if (dev_alloc(ctx, &ctx->h1, (size_t)R * D)) return 1;
     if (dev_alloc(ctx, &ctx->v_net, (size_t)R * ctx->chw)) return 1;
-    if (dev_alloc(ctx, &ctx->rb_count, (M + 255) / 256 + 1)) return 1;
-    {
-        ctx->fin_stride = 4 + (int)((M + 255) / 256) + 4;
-        if (dev_alloc(ctx, &ctx->fin_ctl, (size_t)2 * ctx->fin_stride)) return 1;
-        std::vector<int> init((size_t)2 * ctx->fin_stride, -1);
-        for (int sset = 0; sset < 2; ++sset)
-            for (int i = 0; i < 4; ++i) init[(size_t)sset * ctx->fin_stride + i] = 0;
-        CUDA_OK(cudaMemcpy(ctx->fin_ctl, init.data(), init.size() * sizeof(int), cudaMemcpyHostToDevice));
-    }
     if (alloc_solver_state(ctx, R)) return 1;
 
-    // default: the CTA-pair kernel for every token-level GEMM (LFM_BN_* = 128 / 256 selects the 1-CTA kernel)
-    ctx->bn_qkv = pick_bn(3 * D, "LFM_BN_QKV", kGemmPair);
-    ctx->bn_proj = pick_bn(D, "LFM_BN_PROJ", kGemmPair);
-    ctx->bn_fc1 = pick_bn(Hd, "LFM_BN_FC1", kGemmPair);
-    ctx->bn_fc2 = pick_bn(D, "LFM_BN_FC2", kGemmPair);
-    ctx->bn_mod = 256;
     bool ok = true;
-    ok &= make_tmap_bf16(&ctx->tm_xn, ctx->xn, M, D, 128);
-    ok &= make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, 128);
-    ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, 128);
-    ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, 128);
-    ok &= make_tmap_bf16(&ctx->tm_qkv_q, ctx->qkv, M, 3 * Dq, 128);
-    ok &= make_tmap_bf16(&ctx->tm_qkv_kv, ctx->qkv, M, 3 * Dq, 256);
-    ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, ctx->bn_mod);
-    ok &= make_tmap_bf16(&ctx->tm64_xn, ctx->xn, M, D, 64);
-    ok &= make_tmap_bf16(&ctx->tm64_attn, ctx->attn, M, Dq, 64);
-    ok &= make_tmap_bf16(&ctx->tm64_hmid, ctx->hmid, M, Hd, 64);
-    ok &= make_tmap_out(&ctx->tmo_qkv, ctx->qkv, M, 3 * Dq, false);
-    ok &= make_tmap_out(&ctx->tmo_hmid, ctx->hmid, M, Hd, false);
-    ok &= make_tmap_out(&ctx->tmo_xtok, ctx->x_tok, M, D, true);
+    ok &= make_tmap_bf16(&ctx->tm_xn, ctx->xn, M, D, kGemmBoxRows);
+    ok &= make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, kGemmBoxRows);
+    ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, kGemmBoxRows);
+    ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
+    ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, kGemmBoxRows);
+    if (!ctx->qkv_head_major) ok &= make_tmap_bf16(&ctx->tm_qkv_attn, ctx->qkv, M, 3 * Dq, kGemmBoxRows);
     for (auto& b : ctx->blk) {
-        ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, weight_box_rows(ctx->bn_qkv));
-        ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, weight_box_rows(ctx->bn_proj));
-        ok &= make_tmap_bf16(&b.tm_fc1, b.w_fc1, Hd, D, weight_box_rows(ctx->bn_fc1));
-        ok &= make_tmap_bf16(&b.tm_fc2, b.w_fc2, D, Hd, weight_box_rows(ctx->bn_fc2));
-        ok &= make_tmap_bf16(&b.tmh_qkv, b.w_qkv, 3 * Dq, D, 64);
-        ok &= make_tmap_bf16(&b.tmh_proj, b.w_proj, D, Dq, 64);
-        ok &= make_tmap_bf16(&b.tmh_fc1, b.w_fc1, Hd, D, 64);
-        ok &= make_tmap_bf16(&b.tmh_fc2, b.w_fc2, D, Hd, 64);
+        ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, kGemmBoxRows);
+        ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, kGemmBoxRows);
+        ok &= make_tmap_bf16(&b.tm_fc1, b.w_fc1, Hd, D, kGemmBoxRows);
+        ok &= make_tmap_bf16(&b.tm_fc2, b.w_fc2, D, Hd, kGemmBoxRows);
     }
     if (!ok) return fail(ctx, "lfm_finalize: cuTensorMapEncodeTiled failed");
     ctx->max_rows = R;
@@ -868,7 +638,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     LAUNCH_OK();
     {   // all adaLN modulation vectors of the network in one GEMM: mod[crows, (6L+2) D]
         GemmEpi ep{ctx->b_mod, ctx->mod, ctx->Nmod, nullptr, 0, 1};
-        CUDA_OK(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, ctx->bn_mod, ep));
+        CUDA_OK(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
         ctx->launches++;
     }
     const int ps = ctx->d.patch_size;
@@ -890,92 +660,53 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         dir ^= 1;
         return d;
     };
-    // LayerNorm fusion: the proj / fc2 GEMMs (pair kernel, full rows: N == D) also emit the LayerNorm-modulated operand of
-    // the layer that follows them; only the very first LayerNorm of the network is a stand-alone pass.
-    const bool fuse = ctx->ln_fuse && ctx->bn_proj == kGemmPair && ctx->bn_fc2 == kGemmPair;  // (the finisher lives in gemm2 only)
-    int fin_set = 0;  // the 2 L finisher launches of one evaluation alternate between the two control blocks, starting at 0
-    static const int g2_flags = env_int("LFM_G2_FLAGS", 0) & 8;  // 8: bf16 epilogues store straight from registers (A/B switch)
     for (int l = 0; l < L; ++l) {
         BlockW& b = ctx->blk[l];
         const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
-        if (l == 0 || !fuse) {
+        {
             const int d = next_dir();
             CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, (zig ? 1 + d : 0) | (ctx->l2_hint ? 4 : 0)));
             ctx->launches++;
         }
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
-            ep.dbg_flags = g2_flags;
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, ctx->bn_qkv, ep, &ctx->tmo_qkv, &b.tmh_qkv, &ctx->tm64_xn));
+            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, 0, ep));
             ctx->launches++;
         }
         {
-            const int d = next_dir();
-            if (ctx->qkv_head_major) {  // mma.sync kernels on head-major qkv rows (see lfm_create)
-                // head_dim 64 keeps the kernel's own ch^-1/2; the padded DiT-XL heads pass the true head_dim^-1/2
-                const float sc = 1.4426950408889634f / sqrtf(static_cast<float>(ctx->dh));
-                if (T == 16 || T == 64)   // 4 x 4 / 8 x 8 token grids: the whole sequence in registers
-                    CUDA_OK(launch_attention_mma(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, ctx->dh == 64 ? 0.f : sc));
-                else                      // 256 tokens with head_dim 72, 1024 tokens: keys streamed in chunks of 64
-                    CUDA_OK(launch_attention_flash(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, sc));
-            } else if (ctx->attn_variant >= 2)
-                CUDA_OK(launch_attention2(s, ctx->tm_qkv_kv, ctx->tm_attn, rows, ctx->H, D, ctx->attn_variant, d));
-            else if (ctx->attn_variant == 0)
-                CUDA_OK(launch_attention_inst<true>(s, ctx->tm_qkv_q, ctx->tm_qkv_kv, ctx->attn, rows, ctx->H, D, nullptr));
-            else
-                CUDA_OK(launch_attention_inst<false>(s, ctx->tm_qkv_q, ctx->tm_qkv_kv, ctx->attn, rows, ctx->H, D, nullptr));
+            next_dir();  // attention reads each (sample, head) once: the sweep direction only keeps the GEMMs alternating
+            // head_dim 64 keeps the kernel's own ch^-1/2; the padded DiT-XL heads pass the true head_dim^-1/2
+            const float sc = 1.4426950408889634f / sqrtf(static_cast<float>(ctx->dh));
+            if (!ctx->qkv_head_major)                          // 256 tokens, head_dim 64: TMA + wgmma
+                CUDA_OK(launch_attention_wgmma(s, ctx->tm_qkv_attn, ctx->attn, Dq, ctx->H, rows));
+            else if (T == 16 || T == 64)                       // 4 x 4 / 8 x 8 token grids: the whole sequence in registers
+                CUDA_OK(launch_attention_mma(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, ctx->dh == 64 ? 0.f : sc));
+            else                                               // 1024 tokens, head_dim 72: keys streamed in chunks of 64
+                CUDA_OK(launch_attention_flash(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, sc, false));
             ctx->launches++;
         }
         {
-            GemmEpi ep{b.b_proj, ctx->x_tok, D, mb + 2 * D, Nmod, T};
+            GemmEpi ep{b.b_proj, ctx->x_tok, D, mb + 2 * D, Nmod, T};  // x += gate_msa * proj(...)   (models/DiT.py:129)
             ep.reverse_m = next_dir();
-            ep.l2_keep = ctx->l2_hint;
-            if (fuse) {  // x += gate_msa * proj(...), then xn = LN(x) * (1 + scale_mlp) + shift_mlp   (models/DiT.py:129-130)
-                ep.rb_count = ctx->rb_count;
-                ep.fin_ctl = ctx->fin_ctl;
-                ep.fin_stride = ctx->fin_stride;
-                ep.fin_set = fin_set;
-                fin_set ^= 1;
-                ep.ln_out = ctx->xn;
-                ep.ln_shift = mb + 3 * D;
-                ep.ln_scale = mb + 4 * D;
-                ep.ln_stride = Nmod;
-            }
-            CUDA_OK(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, ctx->bn_proj, ep, &ctx->tmo_xtok, &b.tmh_proj, &ctx->tm64_attn));
+            CUDA_OK(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
             ctx->launches++;
         }
-        if (!fuse) {
+        {
             const int d = next_dir();
             CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, (zig ? 1 + d : 0) | (ctx->l2_hint ? 4 : 0)));
             ctx->launches++;
         }
         {
             GemmEpi ep{b.b_fc1, ctx->hmid, Hd, nullptr, 0, T};
-            ep.dbg_flags = g2_flags;
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, ctx->bn_fc1, ep, &ctx->tmo_hmid, &b.tmh_fc1, &ctx->tm64_xn));
+            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, 0, ep));
             ctx->launches++;
         }
         {
-            GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};
+            GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};  // x += gate_mlp * fc2(...)   (models/DiT.py:130)
             ep.reverse_m = next_dir();
-            ep.l2_keep = ctx->l2_hint;
-            if (fuse) {  // x += gate_mlp * fc2(...), then the NEXT block's xn = LN(x) * (1 + scale_msa) + shift_msa
-                ep.rb_count = ctx->rb_count;
-                ep.fin_ctl = ctx->fin_ctl;
-                ep.fin_stride = ctx->fin_stride;
-                ep.fin_set = fin_set;
-                fin_set ^= 1;
-                if (l + 1 < L) {  // (the last block's launch only keeps the control blocks alternating: FinalLayer has its own LayerNorm)
-                    const float* mn = ctx->mod + (size_t)(l + 1) * 6 * D;
-                    ep.ln_out = ctx->xn;
-                    ep.ln_shift = mn;
-                    ep.ln_scale = mn + D;
-                    ep.ln_stride = Nmod;
-                }
-            }
-            CUDA_OK(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, ctx->bn_fc2, ep, &ctx->tmo_xtok, &b.tmh_fc2, &ctx->tm64_hmid));
+            CUDA_OK(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
             ctx->launches++;
         }
     }
@@ -1617,44 +1348,37 @@ extern "C" int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float*
                             void* stream) {
     lfm_ctx* ctx = nullptr;
     if (K % 64 != 0 || N % 8 != 0) return fail(ctx, "lfm_dbg_gemm: K must be a multiple of 64 and N of 8");
-    if (block_n != 128 && block_n != 256 && block_n != kGemmPair && block_n != kGemmQuad && block_n != kGemmPair512)
-        return fail(ctx, "lfm_dbg_gemm: block_n must be 128, 256, 512 (CTA pair), 640 (CTA pair, 512 x 256 tile) or 1024 (4-CTA cluster)");
+    if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(ctx, "lfm_dbg_gemm: unknown epilogue %d", epi);
+    if (block_n != 0 && block_n != 128 && block_n != 256 && block_n != 512 && block_n != 640 && block_n != 1024)
+        return fail(ctx, "lfm_dbg_gemm: block_n must be 0, 128, 256, 512, 640 or 1024");
     g_num_sms = query_num_sms();
     if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
     CUtensorMap ta, tb;
-    if (!make_tmap_bf16(&ta, a_bf16, M, K, 128) || !make_tmap_bf16(&tb, w_bf16, N, K, weight_box_rows(block_n)))
+    if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
         return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
     GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
-    ep.dbg_flags = env_int("LFM_G2_DBG", 0);
-    CUtensorMap tout;
-    if (!make_tmap_out(&tout, out, M, N, epi >= 2)) return fail(ctx, "lfm_dbg_gemm: output tensor map encode failed");
-    CUtensorMap tbh;
-    if (!make_tmap_bf16(&tbh, w_bf16, N, K, 64)) return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
-    CUtensorMap ta64;
-    if (!make_tmap_bf16(&ta64, a_bf16, M, K, 64)) return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
-    CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep, &tout, &tbh, &ta64));
+    CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n == 128 || block_n == 256 ? block_n : 0, ep));
     return 0;
 }
 
 extern "C" int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s,
                                  void* stream) {
     lfm_ctx* ctx = nullptr;
-    const int D = H * 64;
-    const uint64_t M = (uint64_t)B * 256;
-    CUtensorMap tq, tkv;
-    if (!make_tmap_bf16(&tq, qkv_bf16, M, 3 * D, 128) || !make_tmap_bf16(&tkv, qkv_bf16, M, 3 * D, 256))
-        return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
+    if (variant != 0 && variant != 1) return fail(ctx, "lfm_dbg_attention: variant must be 0 (wgmma) or 1 (mma.sync flash)");
+    if (dbg_s != nullptr) return fail(ctx, "lfm_dbg_attention: dbg_s is not supported (pass NULL)");
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (variant >= 2) {
-        g_num_sms = query_num_sms();
-        if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-        CUtensorMap tout;
-        if (!make_tmap_bf16(&tout, out_bf16, M, D, 128)) return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
-        CUDA_OK(launch_attention2(s, tkv, tout, B, H, D, variant));
-    } else if (variant == 0)
-        CUDA_OK(launch_attention_inst<true>(s, tq, tkv, static_cast<__nv_bfloat16*>(out_bf16), B, H, D, dbg_s));
-    else
-        CUDA_OK(launch_attention_inst<false>(s, tq, tkv, static_cast<__nv_bfloat16*>(out_bf16), B, H, D, dbg_s));
+    if (variant == 0) {
+        CUtensorMap tq;
+        if (!make_tmap_bf16(&tq, qkv_bf16, (uint64_t)B * 256, (uint64_t)3 * H * 64, kGemmBoxRows))
+            return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
+        CUDA_OK(launch_attention_wgmma(s, tq, static_cast<__nv_bfloat16*>(out_bf16), H * 64, H, B));
+    } else {
+        const float sc = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e), head_dim = 64
+        CUDA_OK(launch_attention_flash(s, static_cast<const __nv_bfloat16*>(qkv_bf16), static_cast<__nv_bfloat16*>(out_bf16), 256, 64,
+                                       H * 64, H, B * H, sc, true));
+    }
     return 0;
 }
 
@@ -1670,7 +1394,7 @@ extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B
     if (T == 16 || T == 64)
         CUDA_OK(launch_attention_mma(s, q, o, T, ch, H * ch, H, B * H, sc));
     else if (T > 0 && T % 64 == 0)
-        CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc));
+        CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
     else
         return fail(ctx, "lfm_dbg_attention_mma: T must be 16 or a multiple of 64 (got %d)", T);
     return 0;

@@ -1,6 +1,6 @@
 // lfm_b200 - non-GEMM kernels of the ADM UNetModel velocity network (reference models/guided_diffusion/unet.py).
 // Activations are NHWC: an fp32 "stream" tensor per block output (skip connections, residual adds) and bf16 operand
-// tensors feeding the tcgen05 implicit-GEMM convolutions (gemm2.cuh with a 4-D TMA im2col producer).
+// tensors feeding the wgmma implicit-GEMM convolutions (gemm.cuh with a 4-D TMA im2col producer).
 #pragma once
 #include <type_traits>
 #include "common.cuh"
@@ -212,8 +212,8 @@ gn_apply_kernel(GnApplyArgs a) {
     }
 }
 
-// The same pass for a bf16 SOURCE of C <= 512 channels (conv1's output H1; no pass-through copies): 8-byte loads per lane kept
-// only half the bytes in flight and ran at 3.6 TB/s where the fp32-source pass reaches 5.5.  Here a warp takes a GROUP of PIXB
+// The same pass for a bf16 SOURCE of C <= 512 channels (conv1's output H1; no pass-through copies): 8-byte loads per lane would keep
+// only half the bytes of the fp32-source pass in flight.  Here a warp takes a GROUP of PIXB
 // consecutive pixels as one contiguous run of 16-byte chunks (8 channels each; chunk t of the group belongs to lane t % 32), eight
 // (six for C = 384) chunks per lane in flight.  HW % PIXB == 0 (checked by the host).
 __host__ __device__ constexpr int gn_apply_bf16_pixels(int J) { return J == 1 ? 16 : J == 2 ? 8 : 4; }
@@ -395,7 +395,7 @@ conv_out_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ W
     }
 }
 
-// out.2 on the tensor cores: the pair GEMM writes [B*H*W, 4] (NHWC); this scatters it to the NCHW velocity.
+// out.2 on the tensor cores: the GEMM writes [B*H*W, 4] (NHWC); this scatters it to the NCHW velocity.
 __global__ void nhwc4_to_nchw_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int HW) {
     pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
     pdl_trigger();
@@ -412,8 +412,7 @@ __global__ void nhwc4_to_nchw_kernel(const float* __restrict__ in, float* __rest
 
 // Upsample: nearest x2 of the fp32 stream -> bf16 operand of the following conv3x3 (unet.py:92-99).
 // One thread per INPUT float4: one 16-byte load, four 8-byte stores (the 2 x 2 output pixels); grid (ceil(W * C/4 / 256), B * H),
-// so the only index arithmetic is one 32-bit division (the first version decoded a flat 64-bit output index per thread: three
-// 64-bit divisions per 8 bytes stored, 2.3 TB/s).
+// so the only index arithmetic is one 32-bit division (not three 64-bit divisions per 8 bytes stored for a flat output index).
 __global__ void __launch_bounds__(256)
 upsample2x_cast_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int H, int W, int C) {
     pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
@@ -596,7 +595,7 @@ attention_small_smem_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16
 
 // ------------------------------------------------------------------------------------------------
 // Attention core for the short token grids (T = 16 or 64 tokens per sample) on the tensor cores: warp-level
-// mma.sync m16n8k16 (bf16 in, fp32 accumulate) - these tiles are far too small for a tcgen05 pipeline, and the SIMT
+// mma.sync m16n8k16 (bf16 in, fp32 accumulate) - these tiles are far too small for a TMA / wgmma pipeline, and the SIMT
 // kernels above are instruction-issue bound (about 1000 warp instructions per query).  Same layouts as
 // attention_small_kernel: qkv [B*T, 3C] with channel = head*3ch + {q,k,v}*ch + c, out [B*T, C].
 // One warp owns 16 query rows: S = Q K^T stays in registers, softmax on the accumulator fragments (fp32), the bf16

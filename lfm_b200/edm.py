@@ -74,7 +74,7 @@ def _unet_block(cin, cout, emb, attention=False, up=False, down=False):
 
 
 class DhariwalUNet(_NativeNet):
-    """B200-native DhariwalUNet with the reference's constructor (models/EDM.py:717-733)."""
+    """H100-native DhariwalUNet with the reference's constructor (models/EDM.py:717-733)."""
 
     def __init__(self, img_resolution, in_channels, out_channels, label_dim=0, augment_dim=0, model_channels=192,
                  channel_mult=(1, 2, 3, 4), channel_mult_emb=4, num_blocks=3, attn_resolutions=(32, 16, 8), dropout=0.10,
@@ -190,7 +190,7 @@ class DhariwalUNet(_NativeNet):
 def get_edm_network(config):
     """reference models/EDM.py:864-937.  Only ``model_type == "adm"`` (the LFM ADM presets) is native."""
     if config.model_type != "adm":
-        raise NotImplementedError(f"model_type '{config.model_type}' (SongUNet / context ADM) is outside the B200 hot path; "
+        raise NotImplementedError(f"model_type '{config.model_type}' (SongUNet / context ADM) is outside the native hot path; "
                                   "'adm' (DhariwalUNet) and the DiT family are native")
     return DhariwalUNet(
         img_resolution=config.image_size // config.f,

@@ -5,7 +5,7 @@ return a :class:`DiT` whose *parameters* are ordinary ``nn.Module`` state (same 
 shapes as the reference - SURVEY.md 8(b) - so ``load_state_dict(ckpt, strict=True)``, ``.parameters()``,
 ``.eval()``, ``.to(device)`` behave identically), and whose *compute* is liblfm_b200.so: ``model(t, x, y)`` and
 ``model.forward_with_cfg(t, x, y, cfg_scale)`` call the C ABI (include/lfm_b200.h) on the current CUDA stream.
-There is no PyTorch implementation of the forward pass in this package and no fallback: without a B200 and the
+There is no PyTorch implementation of the forward pass in this package and no fallback: without an H100 and the
 built library the call raises.
 """
 from __future__ import annotations
@@ -96,7 +96,7 @@ class _NativeNet(nn.Module):
         """Return the lfm_ctx handle, (re)creating it and uploading the weights when needed."""
         lib = _lib.load()
         if device.type != "cuda":
-            raise RuntimeError("lfm_b200 runs on a CUDA device (B200, sm_100a) only; got tensors on " + str(device))
+            raise RuntimeError("lfm_b200 runs on a CUDA device (H100, sm_90a) only; got tensors on " + str(device))
         dev_index = device.index if device.index is not None else torch.cuda.current_device()
         if (self._ctx is not None and not self._dirty and rows <= self._ctx_rows and self._ctx_device == dev_index
                 and self._quick_probe() == self._probe):
@@ -177,7 +177,7 @@ class _NativeNet(nn.Module):
 
 
 class DiT(_NativeNet):
-    """B200-native DiT velocity network with the reference's constructor (models/DiT.py:157-169)."""
+    """H100-native DiT velocity network with the reference's constructor (models/DiT.py:157-169)."""
 
     def __init__(self, img_resolution=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
                  mlp_ratio=4.0, label_dropout=0.1, num_classes=1000, learn_sigma=False, max_batch=None):

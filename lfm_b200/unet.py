@@ -2,7 +2,7 @@
 
 Parameters live in an ``nn.Module`` tree with the reference's ``state_dict`` keys (``time_embed.{0,2}``,
 ``input_blocks.N.M.{in_layers,emb_layers,out_layers,skip_connection,norm,qkv,proj_out,op}``, ``middle_block``,
-``output_blocks``, ``out.{0,2}``); the compute is liblfm_b200.so (tcgen05 implicit-GEMM convolutions, fused
+``output_blocks``, ``out.{0,2}``); the compute is liblfm_b200.so (wgmma implicit-GEMM convolutions, fused
 GroupNorm/SiLU/FiLM, attention).  Only the configuration the LFM presets use is native:
 ``use_scale_shift_norm=True``, ``resblock_updown=False``, ``conv_resample=True``, legacy attention order, dims=2.
 """

@@ -1,4 +1,4 @@
-"""B200-native decoder of the Stable-Diffusion ``AutoencoderKL`` - the VAE decode step of the sampling path
+"""H100-native decoder of the Stable-Diffusion ``AutoencoderKL`` - the VAE decode step of the sampling path
 (``first_stage_model.decode(fake_sample / args.scale_factor).sample``, test_flow_latent.py:131,193;
 test_flow_latent_ddp.py:57,110).
 
@@ -8,7 +8,7 @@ part of its interface the reference uses: ``AutoencoderKL.from_pretrained(dir)``
 ``.decode(z).sample``.  Parameters live in an ``nn.Module`` tree with the diffusers ``state_dict`` keys of the decoder
 (``decoder.*``, ``post_quant_conv.*``; a full checkpoint's ``encoder.*`` / ``quant_conv.*`` entries are ignored, legacy
 attention names are renamed as diffusers does); the compute is liblfm_b200.so (``lfm_create_vae`` / ``lfm_decode``:
-tcgen05 implicit-GEMM convolutions, fused GroupNorm + SiLU, tensor-core attention GEMMs).  ``decode_to_uint8`` also
+wgmma implicit-GEMM convolutions, fused GroupNorm + SiLU, tensor-core attention GEMMs).  ``decode_to_uint8`` also
 fuses the generation loop's post-processing (test_flow_latent_ddp.py:131-135).  No PyTorch forward, no fallback.
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""The four DiT-L/2 GEMM shapes at batch 64 through (a) torch.matmul (cuBLAS) and (b) lfm_dbg_gemm (the CTA-pair tcgen05
+"""The four DiT-L/2 GEMM shapes at batch 64 through (a) torch.matmul (cuBLAS) and (b) lfm_dbg_gemm (the wgmma
 kernel with its fused epilogue), a few launches each - run under ncu to compare kernel names / tile shapes / counters:
   ncu --set full --clock-control none -k regex:'nvjet|cutlass|gemm' -c 24 -o gpurun_out/r2_gemm python scripts/gemm_profile.py"""
 import ctypes as C

@@ -1,5 +1,5 @@
 """The library baseline of bench.py's `gpu_eager_baseline` leg: the reference DiT in plain eager PyTorch on the GPU,
-the way a user of the reference would run it on a B200 - `F.scaled_dot_product_attention` (what timm's Attention
+the way a user of the reference would run it on a GPU - `F.scaled_dot_product_attention` (what timm's Attention
 dispatches to), optional bf16 autocast, TF32 on (test_flow_latent_ddp.py:23).  Self-contained torch.nn.functional
 code over the reference's state_dict keys (models/DiT.py:112-131,252-272; timm PatchEmbed / Attention / Mlp).
 

@@ -1,4 +1,4 @@
-"""Reference-equivalent EAGER PyTorch on the B200 (test tooling; uses the oracle restatement, which is the reference's
+"""Reference-equivalent EAGER PyTorch on the GPU (test tooling; uses the oracle restatement, which is the reference's
 algorithm op for op): DiT-L/2 forward, batch 64, fp32 with TF32 off (test_flow_latent.py:103 leaves TF32 commented
 out), TF32 on (test_flow_latent_ddp.py:23) and bf16 autocast.  Prints NFE*img/s and Euler-50 images/s."""
 import json

@@ -1,4 +1,4 @@
-"""GPU bring-up diagnostics (run on the B200 box):  python tests/tools/gpu_bringup.py <group>
+"""GPU bring-up diagnostics (run on an H100):  python tests/tools/gpu_bringup.py <group>
 Groups: gemm, attn, forward, sampler, perf.  Prints error statistics; used to localise kernel bugs."""
 import ctypes as C
 import os
@@ -95,13 +95,11 @@ def group_attn():
     g = torch.Generator().manual_seed(3)
     qkv = (torch.randn(B * 256, 3 * D, generator=g)).to(dev).bfloat16()
     s_ref, o_ref = attn_ref(qkv, B, H)
-    for variant in (1, 0, 2, 3):
+    for variant in (0, 1):
         out = torch.zeros(B * 256, D, device=dev, dtype=torch.bfloat16)
-        dbg = torch.zeros(B, H, 256, 256, device=dev)
-        rc = lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, P(dbg), None)
+        rc = lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
         torch.cuda.synchronize()
         print(f" attention variant {variant} rc={rc} {_lib.last_error() if rc else ''}")
-        stats("S=QK^T", dbg, s_ref)
         stats("O", out.float(), o_ref)
         # per-q-tile / per-column-block diagnostics
         e = (out.float() - o_ref).abs().reshape(B, 2, 128, H, 64)
@@ -110,7 +108,7 @@ def group_attn():
     D = H * 64
     qkv = (torch.randn(B * 256, 3 * D, generator=g)).to(dev).bfloat16()
     _, o_ref = attn_ref(qkv, B, H)
-    for variant in (0, 1, 2, 3):
+    for variant in (0, 1):
         out = torch.zeros(B * 256, D, device=dev, dtype=torch.bfloat16)
         lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
         torch.cuda.synchronize()

@@ -3,7 +3,7 @@
 // Times lfm::ln_modulate_kernel<8> (M = 16384 rows of 1024 fp32) right after x was (a) written with plain stores, (b) updated with
 // cp.reduce.async.bulk .add.f32 from shared memory (the non-tensor form of the TMA reduce the GEMM uses), (c) updated with red.global.add.f32,
 // (d) just read by the same kernel, (e) after a 512 MB flush.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I lfm_b200/csrc tests/tools/l2_residency.cu -o /tmp/l2res && /tmp/l2res
+//   mkdir -p build && nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I lfm_b200/csrc tests/tools/l2_residency.cu -o build/l2_residency && build/l2_residency
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "common.cuh"
