@@ -188,8 +188,8 @@ int64_t lfm_launch_count(const lfm_ctx* ctx);
 
 /* ---- kernel-level entry points used by the parity tests (tests/test_gpu_parity.py) ------------------- */
 /* C = A[M,K] W[N,K]^T with epilogue `epi` (0 bias->bf16, 1 bias+gelu->bf16, 2 gated residual fp32, 3 bias->fp32).
- * a, w: bf16 device pointers.  block_n: tile width 128 or 256 (128 x block_n tiles); 0, 512, 640 or 1024: the width the network
- * would pick for this shape (the three larger values name tile shapes of earlier builds and are still accepted). */
+ * a, w: bf16 device pointers.  block_n: tile width 128 or 256 (128 x block_n tiles), or 0 for the width the network would
+ * pick for this shape; any other value is rejected. */
 int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
                  int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream);
 /* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer in the timm feature order ({q,k,v} * D + head * 64 + c) -> out [B*256, D]

@@ -76,14 +76,6 @@ LFM_DEVICE void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-LFM_DEVICE void tma_load_2d_hint(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
-                                 uint64_t hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-}
 // 2-D tiled store shared -> global (bulk group completion).
 LFM_DEVICE void tma_store_2d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
@@ -100,10 +92,6 @@ template <int N>
 LFM_DEVICE void tma_store_wait() {
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
-
-constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
-constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
-constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
 
 // ------------------------------------------------------------------------------------------------
 // small math helpers
@@ -140,18 +128,6 @@ LFM_DEVICE float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
-}
-
-// L2 eviction-priority policies for bulk-async (TMA) traffic (the LayerNorm pass's loads of the residual stream with LFM_L2_HINT).
-LFM_DEVICE uint64_t l2_policy_evict_last() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-LFM_DEVICE uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
 }
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-stream-serialization attribute may

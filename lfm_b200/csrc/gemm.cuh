@@ -12,7 +12,7 @@
 //   EPI_BIAS_GELU_BF16  out = bf16(gelu_tanh(acc + bias))            mlp.fc1 + act  (models/DiT.py:122-124)
 //   EPI_GATE_RESID_F32  x  += gate[b] * (acc + bias)   (fp32 stream) attn.proj / mlp.fc2 + gated residual
 //                                                                    (models/DiT.py:129-130)
-//   EPI_BIAS_F32        out = addend + acc + bias (fp32)             adaLN_modulation Linears in one GEMM, convolutions
+//   EPI_BIAS_F32        out = acc + bias (fp32)                      adaLN_modulation Linears in one GEMM, convolutions
 #pragma once
 #include "common.cuh"
 
@@ -38,9 +38,6 @@ struct GemmEpi {
     // Walk the M blocks from the last to the first.  Consecutive kernels of a network alternate direction so that
     // each one starts on the rows its producer touched LAST - the part still resident in L2.
     int reverse_m = 0;
-    // EPI_BIAS_F32: out = addend + acc + bias, the residual connection of a convolutional block (fp32 [M, ldo]; may alias
-    // out) - so that the block's OUTPUT statistics (gn_bins) can be taken in the same epilogue.
-    const float* addend = nullptr;
 };
 constexpr int kGnBinReplicas = 16;
 constexpr double kGnFixScale = 268435456.0;  // 2^28
@@ -346,16 +343,6 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 const bool cok = col < N;  // N is even; a tail narrower than 8 columns (N = 4) ends inside the block
                 const bool w0 = ok0 && cok, w1 = ok1 && cok;
                 float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
-                if (EPI == EPI_BIAS_F32 && ep.addend != nullptr) {
-                    if (w0) {
-                        const float2 a = __ldcg(reinterpret_cast<const float2*>(ep.addend + static_cast<size_t>(row0) * ep.ldo + col));
-                        v0 += a.x, v1 += a.y;
-                    }
-                    if (w1) {
-                        const float2 a = __ldcg(reinterpret_cast<const float2*>(ep.addend + static_cast<size_t>(row1) * ep.ldo + col));
-                        v2 += a.x, v3 += a.y;
-                    }
-                }
                 if (ep.bias != nullptr && cok) {
                     const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
                     v0 += b0, v1 += b1, v2 += b0, v3 += b1;

@@ -128,16 +128,20 @@ patch_embed_kernel(const float* __restrict__ x, int x_rows, const float* __restr
 // ------------------------------------------------------------------------------------------------
 // K5/K9: LayerNorm (no affine, eps 1e-6) + adaLN modulate, fp32 tokens -> bf16 GEMM operand.
 //   y = (x - mean) * rstd * (1 + scale[b]) + shift[b]        (reference models/DiT.py:20-21,119,121,129-130)
-// HBM-bound (reads 4 B, writes 2 B per element).  Persistent blocks; the token rows stream through a 4-stage
-// shared-memory ring filled by 1-D bulk async copies (cp.async.bulk + mbarrier transaction bytes), 8 rows per
-// stage, so loads of later rows are always in flight while the 8 warps normalise the current ones.
-// One warp per row, two-pass statistics in registers, coalesced bf16 stores.
-// 16 warps, one row each per stage: the per-row chain (shared-memory reads -> two warp reductions -> rsqrt -> modulate -> store, ~1500
-// clk with its waits) is latency-bound, so more rows in flight per SM hide more of it (tests/tools/l2_residency.cu times the pass with x
-// in L2 and after a flush).
-// Two shapes are kept for A/B runs (LFM_LN_ROWS = 8 | 16): 8 rows x 4 stages with per-warp modulation loads (round 1), and 16 rows x 3
-// stages with the tile's shift / scale vectors staged next to its rows.
-__host__ __device__ constexpr int ln_stages(int NV, int ROWS) { return ROWS == 8 ? 4 : (NV > 8 ? 2 : 3); }  // 16 rows: 3 x 72 KB at D = 1024
+// HBM-bound (reads 4 B, writes 2 B per element).  Persistent blocks of 16 warps.  The token rows stream through a
+// shared-memory ring filled by 1-D bulk async copies (cp.async.bulk + mbarrier transaction bytes): a stage holds a tile of
+// 16 rows, one per warp, followed by the shift and scale vectors of the tile's sample, so loads of later tiles are in flight
+// while the warps normalise the current one.  One warp per row, two-pass statistics in registers, coalesced bf16 stores.
+// The per-row chain (shared-memory reads -> two warp reductions -> rsqrt -> modulate -> store, ~1500 clk with its waits) is
+// latency-bound, so 16 rows in flight per SM hide more of it (tests/tools/l2_residency.cu times the pass with x in L2 and
+// after a flush).
+// Tiles are dealt round-robin, so the whole grid sweeps M upwards (down = 0) or downwards (down = 1) in time: a sweep that
+// starts where the producer of x finished finds those rows still in L2.
+// rows_per_sample must be a multiple of 16 (launch_ln checks it), so a tile never straddles two samples.
+constexpr int kLnRows = 16;
+__host__ __device__ constexpr int ln_stages(int NV) { return NV > 8 ? 2 : 3; }  // 3 x 72 KB at D = 1024
+// dynamic shared memory of ln_modulate_kernel<NV>: per stage kLnRows rows of x, then the shift and scale vectors
+__host__ __device__ constexpr int ln_smem_bytes(int NV) { return ln_stages(NV) * (kLnRows + 2) * NV * 128 * 4; }
 
 LFM_DEVICE void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -146,42 +150,21 @@ LFM_DEVICE void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, u
                  : "memory");
 }
 
-LFM_DEVICE void bulk_load_1d_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
-                 : "memory");
-}
-
-template <int NV, int kLnRows>  // NV = D / 128 float4 per lane; kLnRows = rows per stage = warps per block
+template <int NV>  // NV = D / 128 float4 per lane
 __global__ void __launch_bounds__(kLnRows * 32, 1)
 ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, const float* __restrict__ shift,
-                   const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int order_flags) {
+                   const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int down) {
     constexpr int D = NV * 128;
-    constexpr int kLnStages = ln_stages(NV, kLnRows);
-    const int order = order_flags & 3;          // tile order (below)
-    const bool keep = (order_flags & 4) != 0;   // x is the residual stream: load with the evict_last L2 policy
-    const uint64_t policy = keep ? l2_policy_evict_last() : 0;
-    // a stage = kLnRows rows of x + the shift and scale vectors of the tile's sample: one copy of the two vectors per tile instead of
-    // one per warp (8 KB per 4 KB row, twice the bytes of x through L2 -> SM).
-    constexpr uint32_t kStageBytes = (kLnRows + (kLnRows == 16 ? 2 : 0)) * D * 4;
-    const bool mod_smem = kLnRows == 16 && rows_per_sample % kLnRows == 0;  // a tile never straddles two samples
+    constexpr int kLnStages = ln_stages(NV);
+    constexpr uint32_t kStageBytes = (kLnRows + 2) * D * 4;
     extern __shared__ __align__(128) uint8_t ln_smem[];
     __shared__ __align__(8) uint64_t full_bar[kLnStages];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_tiles = (M + kLnRows - 1) / kLnRows;
-    // order 0: contiguous tile range per block (keeps one block inside as few samples as possible);
-    // order 1 / 2: tiles dealt round-robin so that the whole grid sweeps M upwards / downwards in time - a sweep that
-    // starts where the producer of x finished finds those rows still in L2
-    const int per = (num_tiles + gridDim.x - 1) / gridDim.x;
-    const int t_begin = blockIdx.x * per;
-    const int t_end = min(num_tiles, t_begin + per);
-    const int my_tiles = order == 0 ? max(0, t_end - t_begin)
-                                    : (num_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
+    const int my_tiles = (num_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
     auto tile_of = [&](int i) {
-        if (order == 0) return t_begin + i;
         const int g = static_cast<int>(blockIdx.x) + i * static_cast<int>(gridDim.x);
-        return order == 2 ? num_tiles - 1 - g : g;
+        return down ? num_tiles - 1 - g : g;
     };
     if (threadIdx.x == 0) {
         for (int s = 0; s < kLnStages; ++s) mbar_init(&full_bar[s], 1);
@@ -191,22 +174,17 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
     __syncthreads();
     pdl_wait();
     pdl_trigger();
-    auto issue = [&](int i) {  // thread 0: load tile t_begin + i into stage i % kLnStages
+    auto issue = [&](int i) {  // thread 0: load tile tile_of(i) and its sample's modulation vectors into stage i % kLnStages
         const int tile = tile_of(i);
         const int rows = min(kLnRows, M - tile * kLnRows);
         const uint32_t bytes = static_cast<uint32_t>(rows) * D * 4;
+        uint8_t* stage = ln_smem + (i % kLnStages) * kStageBytes;
         uint64_t* bar = &full_bar[i % kLnStages];
-        mbar_arrive_expect_tx(bar, bytes + (mod_smem ? 2u * D * 4 : 0u));
-        if (mod_smem) {
-            const size_t boff = static_cast<size_t>(tile * kLnRows / rows_per_sample) * mod_stride;
-            uint8_t* dst = ln_smem + (i % kLnStages) * kStageBytes + kLnRows * D * 4;
-            bulk_load_1d(dst, shift + boff, D * 4, bar);
-            bulk_load_1d(dst + D * 4, scale + boff, D * 4, bar);
-        }
-        if (keep)
-            bulk_load_1d_hint(ln_smem + (i % kLnStages) * kStageBytes, x + static_cast<size_t>(tile) * kLnRows * D, bytes, bar, policy);
-        else
-            bulk_load_1d(ln_smem + (i % kLnStages) * kStageBytes, x + static_cast<size_t>(tile) * kLnRows * D, bytes, bar);
+        mbar_arrive_expect_tx(bar, bytes + 2u * D * 4);
+        const size_t boff = static_cast<size_t>(tile * kLnRows / rows_per_sample) * mod_stride;
+        bulk_load_1d(stage + kLnRows * D * 4, shift + boff, D * 4, bar);
+        bulk_load_1d(stage + (kLnRows + 1) * D * 4, scale + boff, D * 4, bar);
+        bulk_load_1d(stage, x + static_cast<size_t>(tile) * kLnRows * D, bytes, bar);
     };
     if (threadIdx.x == 0)
         for (int i = 0; i < kLnStages && i < my_tiles; ++i) issue(i);
@@ -215,21 +193,8 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
         const int stage = i % kLnStages;
         const uint32_t parity = (i / kLnStages) & 1;
         const int row = tile_of(i) * kLnRows + warp;
-        const bool ok = row < M;
-        // 8-row shape: the modulation vectors come from global memory, requested first so that their latency overlaps the wait
-        float4 shr[kLnRows == 8 ? NV : 1], scr[kLnRows == 8 ? NV : 1];
-        if (kLnRows == 8 && ok) {
-            const size_t boff = static_cast<size_t>(row / rows_per_sample) * mod_stride;
-            const float4* shp = reinterpret_cast<const float4*>(shift + boff);
-            const float4* scp = reinterpret_cast<const float4*>(scale + boff);
-#pragma unroll
-            for (int m = 0; m < (kLnRows == 8 ? NV : 0); ++m) {
-                shr[m] = __ldg(shp + m * 32 + lane);
-                scr[m] = __ldg(scp + m * 32 + lane);
-            }
-        }
         mbar_wait(&full_bar[stage], parity);
-        if (ok) {
+        if (row < M) {
             const float4* xp = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + warp * D * 4);
             float4 v[NV];
             float s = 0.f;
@@ -248,18 +213,9 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
             const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(D) + 1e-6f);
             uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
             const float4* shs = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + kLnRows * D * 4);
-            const size_t boff = static_cast<size_t>(row / rows_per_sample) * mod_stride;
-            const float4* shg = reinterpret_cast<const float4*>(shift + boff);
-            const float4* scg = reinterpret_cast<const float4*>(scale + boff);
 #pragma unroll
             for (int m = 0; m < NV; ++m) {
-                float4 sh, sc;
-                if constexpr (kLnRows == 8) {
-                    sh = shr[m], sc = scr[m];
-                } else {
-                    sh = mod_smem ? shs[m * 32 + lane] : __ldg(shg + m * 32 + lane);
-                    sc = mod_smem ? shs[D / 4 + m * 32 + lane] : __ldg(scg + m * 32 + lane);
-                }
+                const float4 sh = shs[m * 32 + lane], sc = shs[D / 4 + m * 32 + lane];
                 const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
                 const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
                 const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
@@ -269,54 +225,6 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
         }
         __syncthreads();  // every warp has consumed this stage
         if (threadIdx.x == 0 && i + kLnStages < my_tiles) issue(i + kLnStages);
-    }
-}
-
-// The same pass without the shared-memory ring (LFM_LN_ROWS=0): one row per warp straight from global memory into registers, 64
-// registers so that 32 warps are resident per SM (8 independent row chains per scheduler instead of 4), the grid sweeping M in
-// order (upwards, or downwards for order 2).  Same arithmetic in the same order as ln_modulate_kernel: identical results.
-template <int NV, int THREADS = 256, int MINB = 4>
-__global__ void __launch_bounds__(THREADS, MINB)
-ln_modulate_direct_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, const float* __restrict__ shift,
-                          const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int order_flags) {
-    // THREADS = 1024, MINB = 1 (LFM_LN_ROWS=32): the same 32 resident warps per SM as ONE persistent block per SM, which chains
-    // through programmatic dependent launch like the ring version does.
-    constexpr int D = NV * 128;
-    constexpr int WARPS = THREADS / 32;
-    pdl_wait();
-    pdl_trigger();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool down = (order_flags & 3) == 2;
-    for (int r = blockIdx.x * WARPS + warp; r < M; r += gridDim.x * WARPS) {
-        const int row = down ? M - 1 - r : r;
-        const float4* xp = reinterpret_cast<const float4*>(x + static_cast<size_t>(row) * D);
-        const size_t boff = static_cast<size_t>(row / rows_per_sample) * mod_stride;
-        const float4* shp = reinterpret_cast<const float4*>(shift + boff);
-        const float4* scp = reinterpret_cast<const float4*>(scale + boff);
-        uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
-        float4 v[NV];
-#pragma unroll
-        for (int m = 0; m < NV; ++m) v[m] = xp[m * 32 + lane];
-        float s = 0.f;
-#pragma unroll
-        for (int m = 0; m < NV; ++m) s += (v[m].x + v[m].y) + (v[m].z + v[m].w);
-        const float mean = warp_sum(s) / static_cast<float>(D);
-        float ss = 0.f;
-#pragma unroll
-        for (int m = 0; m < NV; ++m) {
-            const float a = v[m].x - mean, b = v[m].y - mean, c = v[m].z - mean, d = v[m].w - mean;
-            ss += (a * a + b * b) + (c * c + d * d);
-        }
-        const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(D) + 1e-6f);
-#pragma unroll
-        for (int m = 0; m < NV; ++m) {
-            const float4 sh = __ldg(shp + m * 32 + lane), sc = __ldg(scp + m * 32 + lane);
-            const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
-            const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
-            const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
-            const float d = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
-            yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
-        }
     }
 }
 

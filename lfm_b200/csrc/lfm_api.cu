@@ -71,11 +71,6 @@ static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint
     return r == CUDA_SUCCESS;
 }
 
-static int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return (v != nullptr && *v != 0) ? atoi(v) : dflt;
-}
-
 // ------------------------------------------------------------------------------------------------
 // kernel launch helpers
 
@@ -106,23 +101,19 @@ static int query_num_sms() {
     return n;
 }
 
-// Launch with (by default; LFM_PDL=0 disables) the programmatic-stream-serialization attribute: see pdl_wait() in common.cuh.
-static int g_pdl = -1;
+// Launch with the programmatic-stream-serialization attribute: see pdl_wait() in common.cuh.
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, unsigned block, size_t smem, cudaStream_t s, Args&&... args) {
-    if (g_pdl < 0) g_pdl = env_int("LFM_PDL", 1);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = dim3(block);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
     cudaLaunchAttribute at[1];
-    if (g_pdl) {
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = 1;
-    }
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 // ONLY for kernels that execute pdl_wait() before their first global-memory access.
@@ -175,40 +166,27 @@ static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUte
     return cudaErrorInvalidValue;
 }
 
-template <int NV, int ROWS>
-static cudaError_t launch_ln_inst2(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
-                                   int mod_stride, int rows_per_sample, int M, int order) {
-    static DevOnce once;
-    const int smem = ln_stages(NV, ROWS) * (ROWS + (ROWS == 16 ? 2 : 0)) * NV * 128 * 4;
-    auto kern = ln_modulate_kernel<NV, ROWS>;
-    if (cudaError_t e = smem_opt_in(once, kern, smem)) return e;
-    const int tiles = (M + ROWS - 1) / ROWS;
-    const int grid = tiles < g_num_sms ? tiles : g_num_sms;
-    return launch_k(kern, dim3(grid), ROWS * 32, smem, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-}
 template <int NV>
 static cudaError_t launch_ln_inst(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
-                                  int mod_stride, int rows_per_sample, int M, int order) {
-    static const int rows = env_int("LFM_LN_ROWS", 16);  // 16-row ring by default; 8 / 0 / 32: the other shapes (A/B runs)
-    if (rows == 16) return launch_ln_inst2<NV, 16>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-    if (rows == 0) {
-        const int blocks = std::min((M + 7) / 8, 4 * g_num_sms);
-        return launch_k(ln_modulate_direct_kernel<NV>, dim3(blocks), 256, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-    }
-    if (rows == 32) {  // one persistent 32-warp block per SM, rows straight from global memory
-        const int blocks = std::min((M + 31) / 32, g_num_sms);
-        return launch_k(ln_modulate_direct_kernel<NV, 1024, 1>, dim3(blocks), 1024, 0, s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-    }
-    return launch_ln_inst2<NV, 8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
+                                  int mod_stride, int rows_per_sample, int M, int down) {
+    static DevOnce once;
+    auto kern = ln_modulate_kernel<NV>;
+    if (cudaError_t e = smem_opt_in(once, kern, ln_smem_bytes(NV))) return e;
+    const int tiles = (M + kLnRows - 1) / kLnRows;
+    const int grid = tiles < g_num_sms ? tiles : g_num_sms;
+    return launch_k(kern, dim3(grid), kLnRows * 32, ln_smem_bytes(NV), s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
 }
+// down = 0 / 1: the grid sweeps the rows upwards / downwards (ln_modulate_kernel).  A 16-row tile must not straddle two
+// samples: rows_per_sample is a multiple of 16 (the DiT token counts are 16, 64, 256 and 1024).
 static cudaError_t launch_ln(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
-                             int mod_stride, int rows_per_sample, int M, int D, int order = 0) {
+                             int mod_stride, int rows_per_sample, int M, int D, int down) {
+    if (rows_per_sample % kLnRows != 0) return cudaErrorInvalidValue;
     switch (D / 128) {
-        case 2: return launch_ln_inst<2>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-        case 3: return launch_ln_inst<3>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-        case 6: return launch_ln_inst<6>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-        case 8: return launch_ln_inst<8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
-        case 9: return launch_ln_inst<9>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, order);
+        case 2: return launch_ln_inst<2>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+        case 3: return launch_ln_inst<3>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+        case 6: return launch_ln_inst<6>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+        case 8: return launch_ln_inst<8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+        case 9: return launch_ln_inst<9>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
         default: return cudaErrorInvalidValue;
     }
 }
@@ -253,8 +231,6 @@ struct lfm_ctx {
     bool finalized = false;
     std::string err;
     int64_t launches = 0;
-    int zigzag = 0;        // LFM_ZIGZAG: alternate the row-sweep direction of consecutive kernels (L2 reuse)
-    int l2_hint = 0;       // LFM_L2_HINT: evict_last L2 policy on the LayerNorm pass's loads of the residual stream
 
     std::unordered_map<std::string, ParamSlot> params;
     std::vector<void*> allocs;
@@ -380,8 +356,6 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->HW = desc->img_resolution;
     ctx->chw = ctx->C * ctx->HW * ctx->HW;
     ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
-    ctx->zigzag = env_int("LFM_ZIGZAG", 1);
-    ctx->l2_hint = env_int("LFM_L2_HINT", 0);
     const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T;
     const int ps = desc->patch_size;
     const int P = ctx->C * ps * ps;  // elements of one patch = out-features of the final linear
@@ -651,12 +625,11 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
                                                                   ctx->G, ctx->C, ps, M);
     }
     LAUNCH_OK();
-    // L2 zig-zag (LFM_ZIGZAG): consecutive kernels sweep the token rows in opposite directions, so each starts on the
-    // rows its producer wrote last (still L2-resident) instead of the rows that were evicted first.
-    const int zig = ctx->zigzag;
+    // L2 zig-zag: consecutive kernels sweep the token rows in opposite directions, so each starts on the rows its
+    // producer wrote last (still L2-resident) instead of the rows that were evicted first.
     int dir = 1;  // patch_embed wrote x_tok upwards
     auto next_dir = [&]() {
-        const int d = zig ? dir : 0;
+        const int d = dir;
         dir ^= 1;
         return d;
     };
@@ -664,8 +637,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         BlockW& b = ctx->blk[l];
         const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
         {
-            const int d = next_dir();
-            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, (zig ? 1 + d : 0) | (ctx->l2_hint ? 4 : 0)));
+            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, next_dir()));
             ctx->launches++;
         }
         {
@@ -693,8 +665,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
             ctx->launches++;
         }
         {
-            const int d = next_dir();
-            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, (zig ? 1 + d : 0) | (ctx->l2_hint ? 4 : 0)));
+            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, next_dir()));
             ctx->launches++;
         }
         {
@@ -831,16 +802,11 @@ static int get_step_graph(lfm_ctx* ctx, int kind, int n_img, bool has_y, float c
         *launches = it->second.launches;
         return 0;
     }
-    if (env_int("LFM_NO_GRAPH", 0)) {
-        *out = nullptr;
-        return 0;
-    }
     // warm the lazily-set function attributes outside of capture
     const int64_t launches_before = ctx->launches;
     if (record_step(ctx, kind, n_img, has_y, cfg_scale)) return 1;
     CUDA_OK(cudaStreamSynchronize(ctx->stream));
     const int launches_per_replay = static_cast<int>(ctx->launches - launches_before);
-    StepState zero{0, 0, 0};
     // (the warm-up advanced the device step counter and state; callers re-initialise both afterwards)
     cudaGraph_t graph = nullptr;
     CUDA_OK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
@@ -852,7 +818,6 @@ static int get_step_graph(lfm_ctx* ctx, int kind, int n_img, bool has_y, float c
     cudaGraphExec_t exec = nullptr;
     CUDA_OK(cudaGraphInstantiate(&exec, graph, 0));
     CUDA_OK(cudaGraphDestroy(graph));
-    (void)zero;
     ctx->graphs[key].exec = exec;
     ctx->graphs[key].launches = launches_per_replay;
     *launches = launches_per_replay;
@@ -957,13 +922,10 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     cudaGraphExec_t g_euler = nullptr, g_heun = nullptr;
     const int n_int = n_grid - 1;
     const int n_heun = method == LFM_METHOD_HEUN ? (heun_corrector_limit < n_int ? (heun_corrector_limit < 0 ? 0 : heun_corrector_limit) : n_int) : 0;
-    const bool graphs = !env_int("LFM_NO_GRAPH", 0);
     if (join_in(ctx, user)) return 1;
     int l_euler = 0, l_heun = 0;
-    if (graphs) {
-        if (n_heun < n_int && get_step_graph(ctx, 0, B_img, has_y, cfg_scale, &g_euler, &l_euler)) return 1;
-        if (n_heun > 0 && get_step_graph(ctx, 1, B_img, has_y, cfg_scale, &g_heun, &l_heun)) return 1;
-    }
+    if (n_heun < n_int && get_step_graph(ctx, 0, B_img, has_y, cfg_scale, &g_euler, &l_euler)) return 1;
+    if (n_heun > 0 && get_step_graph(ctx, 1, B_img, has_y, cfg_scale, &g_heun, &l_heun)) return 1;
     cudaStream_t s = ctx->stream;
     CUDA_OK(cudaMemcpyAsync(ctx->t_grid, t_grid_host, (size_t)n_grid * sizeof(float), cudaMemcpyDefault, s));
     CUDA_OK(cudaMemcpyAsync(ctx->x_state, x_inout, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -974,13 +936,8 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     int64_t nfe = 0;
     for (int i = 0; i < n_int; ++i) {
         const int kind = i < n_heun ? 1 : 0;
-        cudaGraphExec_t g = kind ? g_heun : g_euler;
-        if (g != nullptr) {
-            CUDA_OK(cudaGraphLaunch(g, s));
-            ctx->launches += kind ? l_heun : l_euler;
-        } else {
-            if (record_step(ctx, kind, B_img, has_y, cfg_scale)) return 1;
-        }
+        CUDA_OK(cudaGraphLaunch(kind ? g_heun : g_euler, s));
+        ctx->launches += kind ? l_heun : l_euler;
         nfe += kind ? 2 : 1;
     }
     CUDA_OK(cudaMemcpyAsync(x_inout, ctx->x_state, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -1155,9 +1112,6 @@ static int dp_get_graph(Dopri& d, float atol, float rtol, cudaGraphExec_t* out, 
         *launches = it->second.launches;
         return 0;
     }
-    *out = nullptr;
-    *launches = 0;
-    if (env_int("LFM_NO_GRAPH", 0)) return 0;
     // warm-up run outside of capture (lazily set function attributes); it only writes scratch: ytmp, y1, k2..k7, ratio
     const int64_t before = ctx->launches;
     if (dp_record_step(d, atol, rtol)) return 1;
@@ -1264,12 +1218,8 @@ extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, dou
             for (int j = 0; j <= ns; ++j) hp->coef[ns][j] = (float)tab.c_sol[j] * dt_32;
         for (int j = 0; j <= ns; ++j) hp->cerr[j] = dt_32 * (float)tab.c_err[j];
         CUDA_OK(cudaMemcpyAsync(ctx->dp_dev, hp, sizeof(DpStep), cudaMemcpyHostToDevice, s));
-        if (g_step != nullptr) {
-            CUDA_OK(cudaGraphLaunch(g_step, s));
-            ctx->launches += l_step;
-        } else if (dp_record_step(d, atol_f, rtol_f)) {
-            return 1;
-        }
+        CUDA_OK(cudaGraphLaunch(g_step, s));
+        ctx->launches += l_step;
         CUDA_OK(cudaStreamSynchronize(s));  // the ONE synchronisation of the step: the controller runs on the host in fp64
         d.nfe += ns;
         const float ratio = fabsf(ctx->ratio_host[0]);
@@ -1349,15 +1299,15 @@ extern "C" int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float*
     lfm_ctx* ctx = nullptr;
     if (K % 64 != 0 || N % 8 != 0) return fail(ctx, "lfm_dbg_gemm: K must be a multiple of 64 and N of 8");
     if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(ctx, "lfm_dbg_gemm: unknown epilogue %d", epi);
-    if (block_n != 0 && block_n != 128 && block_n != 256 && block_n != 512 && block_n != 640 && block_n != 1024)
-        return fail(ctx, "lfm_dbg_gemm: block_n must be 0, 128, 256, 512, 640 or 1024");
+    if (block_n != 0 && block_n != 128 && block_n != 256)
+        return fail(ctx, "lfm_dbg_gemm: block_n must be 0, 128 or 256 (got %d)", block_n);
     g_num_sms = query_num_sms();
     if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
     CUtensorMap ta, tb;
     if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
         return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
     GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
-    CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n == 128 || block_n == 256 ? block_n : 0, ep));
+    CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
     return 0;
 }
 

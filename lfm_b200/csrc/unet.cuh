@@ -497,7 +497,7 @@ attention_small_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __r
 
 // Split-K epilogue: out[m, n] (+)= bias[n] + sum_s partial[s][m][n], slabs added in a fixed order (deterministic).
 __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int S, size_t slab /*elements*/, const float* __restrict__ bias,
-                                     float* out, int N, size_t n4, int accumulate, const float* addend /* nullable; may alias out */) {
+                                     float* out, int N, size_t n4, int accumulate) {
     pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
     pdl_trigger();
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -509,10 +509,6 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int S, s
         acc.x += v.x, acc.y += v.y, acc.z += v.z, acc.w += v.w;
     }
     float4* op = reinterpret_cast<float4*>(out) + i;
-    if (addend != nullptr) {
-        const float4 a = *(reinterpret_cast<const float4*>(addend) + i);
-        acc.x += a.x, acc.y += a.y, acc.z += a.z, acc.w += a.w;
-    }
     if (accumulate) {
         const float4 o = *op;
         acc.x += o.x, acc.y += o.y, acc.z += o.z, acc.w += o.w;

@@ -43,5 +43,4 @@ for B in batches:
     ms = sorted(times)[len(times) // 2]
     per = ms / net.last_stats["nfe"]
     tf = f", {B * FLOPS / per / 1e9:.0f} TFLOP/s" if FLOPS else ""
-    print(f"{mt} Euler-{nfe} batch {B}: {ms:.2f} ms per call, {per:.3f} ms/NFE, {B / ms * 1e3:.1f} img/s{tf} "
-          f"(LFM_GEMM_SPLIT={os.environ.get('LFM_GEMM_SPLIT', '1')})", flush=True)
+    print(f"{mt} Euler-{nfe} batch {B}: {ms:.2f} ms per call, {per:.3f} ms/NFE, {B / ms * 1e3:.1f} img/s{tf}", flush=True)

@@ -26,7 +26,7 @@ for name, N, K, epi in (("qkv", 3072, 1024, 0), ("proj", 1024, 1024, 2), ("fc1",
         c = a @ w.t()
     torch.cuda.synchronize()
     for _ in range(reps):
-        rc = lib.lfm_dbg_gemm(a.data_ptr(), w.data_ptr(), bias.data_ptr(), o.data_ptr(), gate.data_ptr(), N, 256, M, N, K, epi, 512, None)
+        rc = lib.lfm_dbg_gemm(a.data_ptr(), w.data_ptr(), bias.data_ptr(), o.data_ptr(), gate.data_ptr(), N, 256, M, N, K, epi, 0, None)
         assert rc == 0, _lib.last_error()
     torch.cuda.synchronize()
     print(name, "done", flush=True)

@@ -64,13 +64,15 @@ def make_big(model_type, dev, num_classes, label_dropout, max_batch):
     (128, 128, 64, 3, 128), (256, 512, 1024, 0, 256), (512, 1024, 1024, 1, 256), (512, 1024, 4096, 2, 256),
     (512, 1024, 4096, 2, 128), (64, 2048, 1024, 3, 256), (4, 1024, 256, 3, 256), (256, 1152, 384, 0, 256),
     (256, 1152, 384, 1, 128), (16384, 3072, 1024, 0, 256), (16384, 1024, 1024, 2, 128),
-    # block_n 512 / 1024 / 640: the tile width the network picks for the shape (128 x 256, or 128 x 128 when the launch is tile-starved),
+    # the width the network does not pick for the shape, incl. N tails and M tails
+    (512, 256, 64, 3, 256), (768, 1152, 384, 0, 256), (1280, 768, 256, 1, 256), (4096, 1024, 1024, 2, 128),
+    (16384, 4096, 1024, 0, 128), (38 * 512, 512, 128, 3, 128),
+    # block_n 0: the tile width the network picks for the shape (128 x 256, or 128 x 128 when the launch is tile-starved),
     # incl. N tails and M tails
-    (256, 256, 64, 3, 512), (768, 1152, 384, 0, 512), (512, 1024, 4096, 2, 512), (16384, 1024, 4096, 2, 512),
-    (16384, 3072, 1024, 1, 512), (768, 768, 384, 1, 1024), (512, 1024, 4096, 2, 1024), (16384, 3072, 1024, 0, 1024),
-    (512, 256, 64, 3, 640), (256, 256, 128, 3, 640), (768, 1152, 384, 0, 640), (1280, 768, 256, 1, 640), (512, 1024, 4096, 2, 640),
-    (4096, 1024, 1024, 2, 640), (16384, 1024, 4096, 2, 640), (16384, 3072, 1024, 1, 640), (16384, 4096, 1024, 0, 640),
-    (32768, 1024, 1024, 2, 640), (38 * 512, 512, 128, 3, 640)])
+    (256, 256, 64, 3, 0), (768, 1152, 384, 0, 0), (512, 1024, 4096, 2, 0), (16384, 1024, 4096, 2, 0),
+    (16384, 3072, 1024, 1, 0), (768, 768, 384, 1, 0), (16384, 3072, 1024, 0, 0), (512, 256, 64, 3, 0), (256, 256, 128, 3, 0),
+    (1280, 768, 256, 1, 0), (4096, 1024, 1024, 2, 0), (16384, 4096, 1024, 0, 0), (32768, 1024, 1024, 2, 0),
+    (38 * 512, 512, 128, 3, 0)])
 def test_gemm_epilogues(dev, M, N, K, epi, bn):
     lib = _lib.load()
     g = torch.Generator().manual_seed(M + N + K + epi)

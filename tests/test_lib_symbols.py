@@ -64,3 +64,6 @@ def test_unsupported_shapes_are_rejected(lib):
     bad = _lib.ModelDesc(0, 128, 2, 4, 1024, 24, 16, 4096, 1)  # 128 x 128 latents with patch 2: 4096 tokens, not implemented
     assert lib.lfm_create(ctypes.byref(bad), 0, ctypes.byref(ctx)) != 0
     assert "token grid" in _lib.last_error()
+    # GEMM tile widths are 128 and 256 (0: the network's pick); anything else is refused before the device is touched
+    assert lib.lfm_dbg_gemm(None, None, None, None, None, 0, 1, 128, 128, 64, 3, 640, None) != 0
+    assert "block_n" in _lib.last_error()

@@ -65,19 +65,18 @@ def group_gemm():
                                (512, 1024, 4096, 2, 128), (64, 2048, 1024, 3, 256), (4, 1024, 256, 3, 256),
                                (256, 1152, 384, 0, 256), (256, 1152, 384, 0, 128), (16384, 3072, 1024, 0, 256),
                                (16384, 1024, 1024, 2, 128),
-                               (256, 256, 64, 3, 512), (256, 512, 1024, 0, 512), (512, 1024, 1024, 1, 512),
-                               (512, 1024, 4096, 2, 512), (64, 2048, 1024, 3, 512), (768, 1152, 384, 0, 512),
-                               (16384, 3072, 1024, 0, 512), (16384, 1024, 4096, 2, 512), (16384, 4096, 1024, 1, 512)]:
+                               (256, 256, 64, 3, 0), (256, 512, 1024, 0, 0), (512, 1024, 1024, 1, 0),
+                               (512, 1024, 4096, 2, 0), (64, 2048, 1024, 3, 0), (768, 1152, 384, 0, 0),
+                               (16384, 3072, 1024, 0, 0), (16384, 1024, 4096, 2, 0), (16384, 4096, 1024, 1, 0)]:
         gemm_case(M, N, K, epi, bn)
 
 
 def group_gemm4():
     for (M, N, K, epi) in [(256, 512, 64, 3), (256, 512, 1024, 0), (512, 1024, 4096, 2), (768, 768, 384, 1), (16384, 3072, 1024, 0),
                            (16384, 1024, 4096, 2), (16384, 4096, 1024, 1), (16384, 1024, 1024, 2)]:
-        gemm_case(M, N, K, epi, 1024)
+        gemm_case(M, N, K, epi, 0)
     for (N, K, epi) in ((3072, 1024, 0), (1024, 1024, 2), (4096, 1024, 1), (1024, 4096, 2)):
-        for bn in (1024, 512):
-            time_gemm(16384, N, K, epi, bn)
+        time_gemm(16384, N, K, epi, 0)
 
 
 def attn_ref(qkv, B, H):
@@ -266,16 +265,14 @@ def time_gemm(M, N, K, epi, bn, iters=20):
 
 
 def group_perf16k():
-    bn = int(os.environ.get("LFM_PERF_BN", "640"))
     for (N, K, epi) in ((3072, 1024, 0), (1024, 1024, 2), (4096, 1024, 1), (1024, 4096, 2)):
-        time_gemm(16384, N, K, epi, bn)
+        time_gemm(16384, N, K, epi, 0)
 
 
 def group_perf():
     for M in (16384, 32768, 4096):
         for (N, K, epi) in ((3072, 1024, 0), (1024, 1024, 2), (4096, 1024, 1), (1024, 4096, 2)):
-            for bn in (640, 512):
-                time_gemm(M, N, K, epi, bn)
+            time_gemm(M, N, K, epi, 0)
     # cuBLAS reference for the same shapes
     for (M, N, K) in ((16384, 3072, 1024), (16384, 1024, 1024), (16384, 4096, 1024), (16384, 1024, 4096)):
         a = torch.randn(M, K, device=dev).bfloat16(); w = torch.randn(N, K, device=dev).bfloat16()

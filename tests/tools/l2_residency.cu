@@ -1,16 +1,13 @@
 // Micro-benchmark (measurement aid, not part of the library): does the residual stream x stay in L2 after the way the proj / fc2
 // epilogue updates it (bulk reduce-add performed at L2), so that the LayerNorm pass that follows could read it from there?
-// Times lfm::ln_modulate_kernel<8> (M = 16384 rows of 1024 fp32) right after x was (a) written with plain stores, (b) updated with
-// cp.reduce.async.bulk .add.f32 from shared memory (the non-tensor form of the TMA reduce the GEMM uses), (c) updated with red.global.add.f32,
-// (d) just read by the same kernel, (e) after a 512 MB flush.
+// Times lfm::ln_modulate_kernel<8> (M = 16384 rows of 1024 fp32), sweeping the rows upwards and then downwards, right after x was
+// (a) written with plain stores, (b) updated with cp.reduce.async.bulk .add.f32 from shared memory (the non-tensor form of the TMA
+// reduce the GEMM uses), (c) updated with red.global.add.f32, (d) just read by the same kernel, (e) after a 512 MB flush.
 //   mkdir -p build && nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I lfm_b200/csrc tests/tools/l2_residency.cu -o build/l2_residency && build/l2_residency
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "common.cuh"
 #include "kernels.cuh"
-#ifndef LN_ROWS
-#define LN_ROWS 16
-#endif
 
 using namespace lfm;
 
@@ -50,15 +47,14 @@ int main() {
     cudaMemset(x, 0, n * 4);
     int dev = 0, sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    constexpr int kLnRows = LN_ROWS, kLnThreads = LN_ROWS * 32;
-    const int smem = ln_stages(8, kLnRows) * (kLnRows + (kLnRows == 16 ? 2 : 0)) * D * 4;
-    auto kern = ln_modulate_kernel<8, kLnRows>;
+    const int smem = ln_smem_bytes(8);
+    auto kern = ln_modulate_kernel<8>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
     const char* names[] = {"plain stores", "cp.reduce.async.bulk add", "red.global.add.v4.f32", "LayerNorm itself (x just read)", "512 MB flush"};
-    for (int order = 0; order < 3; order += 2)
+    for (int down = 0; down < 2; ++down)
         for (int w = 0; w < 5; ++w) {
             float best = 1e9f, sum = 0.f;
             for (int rep = 0; rep < 7; ++rep) {
@@ -67,18 +63,18 @@ int main() {
                     case 0: write_plain<<<sms * 8, 256>>>(reinterpret_cast<float4*>(x), n / 4, 0.5f); break;
                     case 1: update_bulk_reduce<<<sms * 4, 128>>>(x, n, 0.25f); break;
                     case 2: update_red<<<sms * 8, 256>>>(x, n, 0.25f); break;
-                    case 3: kern<<<sms, kLnThreads, smem>>>(x, y, mod, mod + D, 2 * D, 256, M, 0); break;
+                    case 3: kern<<<sms, kLnRows * 32, smem>>>(x, y, mod, mod + D, 2 * D, 256, M, down); break;
                     default: break;
                 }
                 cudaEventRecord(e0);
-                kern<<<sms, kLnThreads, smem>>>(x, y, mod, mod + D, 2 * D, 256, M, order);
+                kern<<<sms, kLnRows * 32, smem>>>(x, y, mod, mod + D, 2 * D, 256, M, down);
                 cudaEventRecord(e1);
                 cudaEventSynchronize(e1);
                 float ms;
                 cudaEventElapsedTime(&ms, e0, e1);
                 if (rep > 0) { best = ms < best ? ms : best; sum += ms; }
             }
-            printf("ln_modulate<8> (tile order %d) after %-32s: best %.1f us, mean %.1f us\n", order, names[w], best * 1e3f, sum / 6 * 1e3f);
+            printf("ln_modulate<8> (%-4s) after %-32s: best %.1f us, mean %.1f us\n", down ? "down" : "up", names[w], best * 1e3f, sum / 6 * 1e3f);
         }
     cudaError_t e = cudaDeviceSynchronize();
     printf("status: %s\n", cudaGetErrorString(e));
