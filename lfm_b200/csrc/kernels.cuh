@@ -352,29 +352,22 @@ __global__ void cfg_combine_kernel(const float* __restrict__ v_net, float* __res
 }
 
 // ------------------------------------------------------------------------------------------------
-// K13: fixed-step solver updates.  The step schedule lives in device memory (t_grid) and the step index in
-// a device counter, so one captured CUDA graph serves every step of a trajectory with no host involvement.
+// K13: fixed-step solver updates.  The nodes t_grid, a table of every step's S stage times (S = 1 Euler, 2 Heun and
+// midpoint, 4 rk4; built and perturbed on the host) and the step index live in device memory, so one captured CUDA
+// graph serves every step of a trajectory with no host involvement.  The update kernels read dt = t[i+1] - t[i] from
+// the nodes at the counter; step_advance_kernel, the last kernel of a step graph, bumps it.
 struct StepState {
-    int step;         // current interval index i
-    int n_intervals;  // len(t_grid) - 1
-    int perturb;      // torchdiffeq options["perturb"]: the step's first evaluation sees t one fp32 ulp past the node
+    int step;  // current interval index i
 };
 
-// Writes the model time(s) for the next evaluation: t_eval[0] = t_grid[step + which] (which: 0 = t_cur, 1 = t_next)
-__global__ void step_time_kernel(const float* __restrict__ t_grid, const StepState* __restrict__ st, int which,
-                                 float* __restrict__ t_eval) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        float t = t_grid[st->step + which];
-        // Perturb.NEXT in torchdiffeq's negated time s = -t (nextafter(s, s + 1)) = one ulp DOWN in model time
-        if (st->perturb && which == 0) t = nextafterf(t, t - 1.0f);
-        t_eval[0] = t;
-    }
+// t_eval[0..S) = the stage times of interval `step`: t_stage[step * S + j]
+__global__ void stage_time_kernel(const float* __restrict__ t_stage, const StepState* __restrict__ st, int S,
+                                  float* __restrict__ t_eval) {
+    if (blockIdx.x == 0 && static_cast<int>(threadIdx.x) < S) t_eval[threadIdx.x] = t_stage[st->step * S + threadIdx.x];
 }
 
 // Euler:  x <- x + v * (sign * (t[i+1] - t[i]))      (karras_sample.py:116-117; torchdiffeq y0 + dt*f with the
 // reversed-time sign folded in: there dt = s[i+1]-s[i] = -(t[i+1]-t[i]) and f = -v, the same product)
-// advance != 0 bumps the device step counter (done by thread 0 of block 0 AFTER reading it - every block reads
-// the counter before any block can finish, because the increment happens in a separate tiny kernel).
 __global__ void euler_update_kernel(float* __restrict__ x, const float* __restrict__ v, const float* __restrict__ t_grid,
                                     const StepState* __restrict__ st, size_t n) {
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -393,21 +386,16 @@ __global__ void heun_predict_kernel(const float* __restrict__ x, const float* __
     x_pred[i] = x[i] + dt * d_cur[i];
 }
 
-// Heun corrector: x <- x + dt * (0.5 d_cur + 0.5 d_prime) if step < corrector_limit else x <- x_pred
-// (karras_sample.py:155-159; the guard `i < steps - 1` with the reference's never-overridden default steps = 40)
+// Heun corrector: x <- x + dt * (0.5 d_cur + 0.5 d_prime)     (karras_sample.py:155-159; the intervals past the
+// reference's corrector guard replay an Euler step instead)
 __global__ void heun_correct_kernel(float* __restrict__ x, const float* __restrict__ d_cur,
-                                    const float* __restrict__ d_prime, const float* __restrict__ x_pred,
-                                    const float* __restrict__ t_grid, const StepState* __restrict__ st,
-                                    int corrector_limit, size_t n) {
+                                    const float* __restrict__ d_prime, const float* __restrict__ t_grid,
+                                    const StepState* __restrict__ st, size_t n) {
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int step = st->step;
-    if (step < corrector_limit) {
-        const float dt = t_grid[step + 1] - t_grid[step];
-        x[i] = x[i] + dt * (0.5f * d_cur[i] + 0.5f * d_prime[i]);
-    } else {
-        x[i] = x_pred[i];
-    }
+    const float dt = t_grid[step + 1] - t_grid[step];
+    x[i] = x[i] + dt * (0.5f * d_cur[i] + 0.5f * d_prime[i]);
 }
 
 __global__ void step_advance_kernel(StepState* st) {
@@ -424,16 +412,6 @@ struct RkCoef {   // passed by value as a kernel argument: no device upload, no 
 };
 __global__ void set_scalar_kernel(float* dst, float v) {
     if (threadIdx.x == 0 && blockIdx.x == 0) dst[0] = v;
-}
-
-// y_out = y0 + sum_j (coef[j]) * k[j],  coef already multiplied by dt (fp32) on the host
-__global__ void rk_combine_kernel(const float* __restrict__ y0, RkPtrs kp, int nk, RkCoef coef,
-                                  float* __restrict__ y_out, size_t n) {
-    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float acc = 0.f;
-    for (int j = 0; j < nk; ++j) acc = fmaf(kp.k[j][i], coef.c[j], acc);
-    y_out[i] = y0[i] + acc;
 }
 
 // One attempted dopri5 step's numbers, uploaded once per step (the captured step graph reads them from device memory):
@@ -528,7 +506,7 @@ __global__ void dopri_interp_kernel(const float* __restrict__ y0, const float* _
 }
 
 // torchdiffeq fixed-grid midpoint / rk4 (3/8 rule, rk4_alt_step_func) stage arithmetic, written in the same
-// operation order as the Python expressions (real-time form: dt = t1 - t0, k = v).
+// operation order as the Python expressions (real-time form: dt = t1 - t0 read from the nodes at the step counter, k = v).
 //   mode 0: out = y0 + k1 * h                        (midpoint: h = 0.5 dt)
 //   mode 1: out = y0 + dt * k2                       (midpoint result)
 //   mode 2: out = y0 + (dt * k1) * (1/3)
@@ -537,13 +515,15 @@ __global__ void dopri_interp_kernel(const float* __restrict__ y0, const float* _
 //   mode 5: out = y0 + ((k1 + 3 (k2 + k3)) + k4) * dt * 0.125
 __global__ void fixed_rk_stage_kernel(int mode, const float* y0 /*may alias out*/, const float* __restrict__ k1,
                                       const float* __restrict__ k2, const float* __restrict__ k3,
-                                      const float* __restrict__ k4, float dt, float* out, size_t n) {
+                                      const float* __restrict__ k4, const float* __restrict__ t_grid,
+                                      const StepState* __restrict__ st, float* out, size_t n) {
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const float dt = t_grid[st->step + 1] - t_grid[st->step];
     const float third = static_cast<float>(1.0 / 3.0);
     float r;
     switch (mode) {
-        case 0: r = __fadd_rn(y0[i], __fmul_rn(k1[i], dt)); break;
+        case 0: r = __fadd_rn(y0[i], __fmul_rn(k1[i], __fmul_rn(0.5f, dt))); break;
         case 1: r = __fadd_rn(y0[i], __fmul_rn(dt, k2[i])); break;
         case 2: r = __fadd_rn(y0[i], __fmul_rn(__fmul_rn(dt, k1[i]), third)); break;
         case 3: r = __fadd_rn(y0[i], __fmul_rn(dt, __fsub_rn(k2[i], __fmul_rn(k1[i], third)))); break;

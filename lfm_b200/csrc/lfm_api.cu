@@ -253,8 +253,8 @@ struct lfm_ctx {
     // solver state
     cudaStream_t stream = nullptr;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    float *x_state = nullptr, *x_pred = nullptr, *v_eff = nullptr, *d_prime = nullptr, *t_grid = nullptr,
-          *t_eval = nullptr, *coef = nullptr, *ratio = nullptr, *y_stage = nullptr;
+    float *x_state = nullptr, *x_pred = nullptr, *t_grid = nullptr, *t_stage = nullptr, *t_eval = nullptr,
+          *coef = nullptr, *ratio = nullptr, *y_stage = nullptr;
     float* kbuf[7] = {nullptr};
     double* partial = nullptr;
     long long* y_buf = nullptr;
@@ -501,12 +501,11 @@ static int alloc_solver_state(lfm_ctx* ctx, int R) {
     const size_t nst = (size_t)R * ctx->chw;
     if (dev_alloc(ctx, &ctx->x_state, nst)) return 1;
     if (dev_alloc(ctx, &ctx->x_pred, nst)) return 1;
-    if (dev_alloc(ctx, &ctx->v_eff, nst)) return 1;
-    if (dev_alloc(ctx, &ctx->d_prime, nst)) return 1;
     if (dev_alloc(ctx, &ctx->y_stage, nst)) return 1;
     for (int j = 0; j < 7; ++j)
         if (dev_alloc(ctx, &ctx->kbuf[j], nst)) return 1;
     if (dev_alloc(ctx, &ctx->t_grid, 8192 + 64)) return 1;
+    if (dev_alloc(ctx, &ctx->t_stage, 2 * 8192)) return 1;  // S (n_grid - 1) stage times: Heun's 2 x 8191 at most
     if (dev_alloc(ctx, &ctx->t_eval, 8)) return 1;
     if (dev_alloc(ctx, &ctx->coef, 64)) return 1;
     if (dev_alloc(ctx, &ctx->ratio, 8)) return 1;
@@ -700,15 +699,16 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
 }
 
 // Evaluate the (CFG-combined) velocity of n_img latents in `x` into `v_out` [n_img, C, H, W].
-//   cfg_scale > 1: network batch = 2 n_img rows (labels y[0:n] conditional, y[n:2n] null), v = u + s (c - u).
+//   cfg_scale > 1: network batch = 2 n_img rows (labels y[0:n] conditional, y[n:2n] null), v = u + s (c - u);
+//   dup != 0 writes v into both halves of v_out [2 n_img, C, H, W] (forward_with_cfg returns cat[v, v]).
 static int eval_velocity(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int n_img,
-                         const long long* y, float cfg_scale, float* v_out) {
+                         const long long* y, float cfg_scale, int dup, float* v_out) {
     const size_t n = (size_t)n_img * ctx->chw;
     if (cfg_scale > 1.0f && ctx->arch == LFM_ARCH_UNET && ctx_unet_variant(ctx) == 0)
         return fail(ctx, "UNetModel has no forward_with_cfg (reference models/guided_diffusion/unet.py): cfg_scale must be <= 1");
     if (cfg_scale > 1.0f) {
         if (launch_network(ctx, s, t, t_numel, x, n_img, y, 2 * n_img)) return 1;
-        cfg_combine_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->v_net, v_out, n, cfg_scale, 0);
+        cfg_combine_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->v_net, v_out, n, cfg_scale, dup);
         LAUNCH_OK();
     } else {
         if (launch_network(ctx, s, t, t_numel, x, n_img, y, n_img)) return 1;
@@ -732,27 +732,16 @@ extern "C" int lfm_forward(lfm_ctx* ctx, const float* t, int t_numel, const floa
     if (t_numel != 1 && t_numel != B) return fail(ctx, "lfm_forward: t has %d elements, expected 1 or %d", t_numel, B);
     CUDA_OK(cudaSetDevice(ctx->device));
     g_num_sms = ctx->num_sms;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const long long* yl = reinterpret_cast<const long long*>(y);
-    if (cfg_scale > 1.0f && ctx->arch == LFM_ARCH_UNET && ctx_unet_variant(ctx) == 0)
-        return fail(ctx, "lfm_forward: UNetModel has no forward_with_cfg; cfg_scale must be <= 1");
-    if (cfg_scale > 1.0f) {
-        if (B % 2 != 0) return fail(ctx, "lfm_forward: forward_with_cfg needs an even batch (got %d)", B);
-        // a vector t has 2n entries in the reference; both halves carry the same times (the x halves are identical)
-        const int n_img = B / 2;
-        if (launch_network(ctx, s, t, t_numel, x, n_img, yl, B)) return 1;
-        const size_t n = (size_t)n_img * ctx->chw;
-        cfg_combine_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->v_net, v_out, n, cfg_scale, 1);
-        LAUNCH_OK();
-    } else {
-        if (launch_network(ctx, s, t, t_numel, x, B, yl, B)) return 1;
-        CUDA_OK(cudaMemcpyAsync(v_out, ctx->v_net, (size_t)B * ctx->chw * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    }
-    return 0;
+    const bool cfg = cfg_scale > 1.0f;
+    if (cfg && B % 2 != 0) return fail(ctx, "lfm_forward: forward_with_cfg needs an even batch (got %d)", B);
+    // under CFG a vector t has 2n entries in the reference; both halves carry the same times (the x halves are identical)
+    return eval_velocity(ctx, static_cast<cudaStream_t>(stream), t, t_numel, x, cfg ? B / 2 : B,
+                         reinterpret_cast<const long long*>(y), cfg_scale, 1, v_out);
 }
 
 // ------------------------------------------------------------------------------------------------
-// fixed-step solvers: one captured graph per step kind, replayed from the host with no synchronisation
+// step graphs: each step of a fixed-step solver and each attempted step of an adaptive one is one captured graph,
+// replayed from the host
 
 static int join_in(lfm_ctx* ctx, cudaStream_t user) {
     CUDA_OK(cudaEventRecord(ctx->ev_in, user));
@@ -765,63 +754,80 @@ static int join_out(lfm_ctx* ctx, cudaStream_t user) {
     return 0;
 }
 
-// body of one interval, recorded into ctx->stream (under capture or live)
-static int record_step(lfm_ctx* ctx, int kind /*0 euler, 1 heun (with corrector)*/, int n_img, bool has_y, float cfg_scale) {
-    cudaStream_t s = ctx->stream;
-    const size_t n = (size_t)n_img * ctx->chw;
-    const long long* y = has_y ? ctx->y_buf : nullptr;
-    step_time_kernel<<<1, 32, 0, s>>>(ctx->t_grid, ctx->step_state, 0, ctx->t_eval);
-    LAUNCH_OK();
-    if (eval_velocity(ctx, s, ctx->t_eval, 1, ctx->x_state, n_img, y, cfg_scale, ctx->v_eff)) return 1;
-    if (kind == 0) {
-        euler_update_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->x_state, ctx->v_eff, ctx->t_grid, ctx->step_state, n);
-        LAUNCH_OK();
-    } else {
-        heun_predict_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->x_state, ctx->v_eff, ctx->x_pred, ctx->t_grid,
-                                                          ctx->step_state, n);
-        LAUNCH_OK();
-        step_time_kernel<<<1, 32, 0, s>>>(ctx->t_grid, ctx->step_state, 1, ctx->t_eval);
-        LAUNCH_OK();
-        if (eval_velocity(ctx, s, ctx->t_eval, 1, ctx->x_pred, n_img, y, cfg_scale, ctx->d_prime)) return 1;
-        heun_correct_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->x_state, ctx->v_eff, ctx->d_prime, ctx->x_pred, ctx->t_grid,
-                                                          ctx->step_state, 1 << 30, n);
-        LAUNCH_OK();
-    }
-    step_advance_kernel<<<1, 32, 0, s>>>(ctx->step_state);
-    LAUNCH_OK();
-    return 0;
-}
-
-static int get_step_graph(lfm_ctx* ctx, int kind, int n_img, bool has_y, float cfg_scale, cudaGraphExec_t* out,
-                          int* launches) {
-    char key[128];
-    snprintf(key, sizeof(key), "k%d_n%d_y%d_c%.6f", kind, n_img, has_y ? 1 : 0, cfg_scale > 1.0f ? cfg_scale : 0.f);
+// The graph cached under `key`, or a new one: `record` enqueues one step into ctx->stream.  A warm-up run outside of
+// capture sets the lazily set function attributes and counts the kernels of one replay; a second run is captured.
+// The warm-up runs on the live solver state, so callers initialise that state after this call.
+template <typename Record>
+static int get_graph(lfm_ctx* ctx, const char* key, Record&& record, lfm_ctx::StepGraph* out) {
     auto it = ctx->graphs.find(key);
     if (it != ctx->graphs.end()) {
-        *out = it->second.exec;
-        *launches = it->second.launches;
+        *out = it->second;
         return 0;
     }
-    // warm the lazily-set function attributes outside of capture
     const int64_t launches_before = ctx->launches;
-    if (record_step(ctx, kind, n_img, has_y, cfg_scale)) return 1;
+    if (record()) return 1;
     CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    const int launches_per_replay = static_cast<int>(ctx->launches - launches_before);
-    // (the warm-up advanced the device step counter and state; callers re-initialise both afterwards)
+    lfm_ctx::StepGraph g;
+    g.launches = static_cast<int>(ctx->launches - launches_before);
     cudaGraph_t graph = nullptr;
     CUDA_OK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
-    const int rc = record_step(ctx, kind, n_img, has_y, cfg_scale);
+    const int rc = record();
     cudaError_t e = cudaStreamEndCapture(ctx->stream, &graph);
     ctx->launches = launches_before;
     if (rc) return 1;
     if (e != cudaSuccess) return fail(ctx, "graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t exec = nullptr;
-    CUDA_OK(cudaGraphInstantiate(&exec, graph, 0));
+    CUDA_OK(cudaGraphInstantiate(&g.exec, graph, 0));
     CUDA_OK(cudaGraphDestroy(graph));
-    ctx->graphs[key].exec = exec;
-    ctx->graphs[key].launches = launches_per_replay;
-    *launches = launches_per_replay;
-    *out = exec;
+    ctx->graphs[key] = g;
+    *out = g;
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// fixed-step solvers
+
+// One interval of `method` (LFM_METHOD_*), recorded into ctx->stream.  The interval index is the device counter
+// ctx->step_state: the step copies its S stage times from ctx->t_stage into t_eval[0..S), evaluates the network at
+// t_eval + j into k[j], and the update kernels read dt from the nodes ctx->t_grid.
+static int record_fixed_step(lfm_ctx* ctx, int method, int S, int n_img, bool has_y, float cfg_scale) {
+    cudaStream_t s = ctx->stream;
+    const size_t n = (size_t)n_img * ctx->chw;
+    const long long* y = has_y ? ctx->y_buf : nullptr;
+    const float* tg = ctx->t_grid;
+    const StepState* st = ctx->step_state;
+    float* x = ctx->x_state;
+    float* xs = ctx->x_pred;  // input of the later stages
+    float** k = ctx->kbuf;
+    stage_time_kernel<<<1, 32, 0, s>>>(ctx->t_stage, st, S, ctx->t_eval);
+    LAUNCH_OK();
+    auto eval = [&](int j, const float* xin) {
+        return eval_velocity(ctx, s, ctx->t_eval + j, 1, xin, n_img, y, cfg_scale, 0, k[j]);
+    };
+    auto stage = [&](int mode, float* out) {
+        fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(mode, x, k[0], k[1], k[2], k[3], tg, st, out, n);
+        LAUNCH_OK();
+        return 0;
+    };
+    if (method == LFM_METHOD_EULER) {
+        if (eval(0, x)) return 1;
+        euler_update_kernel<<<blocks_for(n), 256, 0, s>>>(x, k[0], tg, st, n);
+        LAUNCH_OK();
+    } else if (method == LFM_METHOD_HEUN) {
+        if (eval(0, x)) return 1;
+        heun_predict_kernel<<<blocks_for(n), 256, 0, s>>>(x, k[0], xs, tg, st, n);
+        LAUNCH_OK();
+        if (eval(1, xs)) return 1;
+        heun_correct_kernel<<<blocks_for(n), 256, 0, s>>>(x, k[0], k[1], tg, st, n);
+        LAUNCH_OK();
+    } else if (method == LFM_METHOD_MIDPOINT) {
+        if (eval(0, x) || stage(0, xs) || eval(1, xs) || stage(1, x)) return 1;
+    } else {
+        if (eval(0, x) || stage(2, xs) || eval(1, xs) || stage(3, xs) || eval(2, xs) || stage(4, xs) || eval(3, xs) ||
+            stage(5, x))
+            return 1;
+    }
+    step_advance_kernel<<<1, 32, 0, s>>>(ctx->step_state);
+    LAUNCH_OK();
     return 0;
 }
 
@@ -837,108 +843,67 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     if (n_grid < 2 || n_grid > 8192) return fail(ctx, "lfm_sample_fixed: n_grid must be in [2, 8192] (got %d)", n_grid);
     if (x_inout == nullptr || t_grid_host == nullptr) return fail(ctx, "lfm_sample_fixed: null tensor");
     if (cfg_scale > 1.0f && y == nullptr) return fail(ctx, "lfm_sample_fixed: CFG needs labels");
+    const int n_int = n_grid - 1, S = method == LFM_METHOD_EULER ? 1 : method == LFM_METHOD_RK4 ? 4 : 2;
+    if (method >= LFM_METHOD_MIDPOINT && n_int * S > 8192) return fail(ctx, "lfm_sample_fixed: too many stages (%d)", n_int * S);
     CUDA_OK(cudaSetDevice(ctx->device));
     g_num_sms = ctx->num_sms;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     const size_t n = (size_t)B_img * ctx->chw;
     const bool has_y = y != nullptr;
-
-    if (method == LFM_METHOD_MIDPOINT || method == LFM_METHOD_RK4) {
-        // torchdiffeq fixed-grid midpoint / rk4: the stage times of the whole trajectory are computed here in fp32
-        // exactly as the Python expressions do (t0 + dt * (1/3) ...), uploaded once, and the stages are launched
-        // back to back - no host synchronisation inside the loop.
-        if (join_in(ctx, user)) return 1;
-        cudaStream_t s = ctx->stream;
-        const int n_int = n_grid - 1, S = method == LFM_METHOD_RK4 ? 4 : 2;
-        if (n_int * S > 8192) return fail(ctx, "lfm_sample_fixed: too many stages (%d)", n_int * S);
-        std::vector<float> tg(n_grid);
-        CUDA_OK(cudaMemcpy(tg.data(), t_grid_host, n_grid * sizeof(float), cudaMemcpyDefault));
-        std::vector<float> ts((size_t)n_int * S);
-        const float third = (float)(1.0 / 3.0), two_thirds = (float)(2.0 / 3.0);
-        for (int i = 0; i < n_int; ++i) {
-            const float t0 = tg[i], t1 = tg[i + 1], dt = t1 - t0;
-            // options["perturb"]: the first evaluation of a step one ulp past t0 (Perturb.NEXT), rk4's last one ulp before
-            // t1 (Perturb.PREV) - in torchdiffeq's negated time; here in model time the directions flip
-            const float t0e = perturb ? nextafterf(t0, t0 - 1.0f) : t0;
-            if (S == 2) {
-                ts[2 * i] = t0e;
-                ts[2 * i + 1] = t0 + 0.5f * dt;
-            } else {
-                ts[4 * i] = t0e;
-                ts[4 * i + 1] = t0 + dt * third;
-                ts[4 * i + 2] = t0 + dt * two_thirds;
-                ts[4 * i + 3] = perturb ? nextafterf(t1, t1 + 1.0f) : t1;
-            }
-        }
-        CUDA_OK(cudaMemcpyAsync(ctx->t_grid, ts.data(), ts.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-        CUDA_OK(cudaMemcpyAsync(ctx->x_state, x_inout, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        const long long* yb = nullptr;
-        if (has_y) {
-            CUDA_OK(cudaMemcpyAsync(ctx->y_buf, y, (size_t)rows * sizeof(long long), cudaMemcpyDefault, s));
-            yb = ctx->y_buf;
-        }
-        CUDA_OK(cudaStreamSynchronize(s));  // ts is host stack/heap memory
-        float* y0 = ctx->x_state;
-        float* ytmp = ctx->x_pred;
-        float** k = ctx->kbuf;
-        int64_t nfe = 0;
-        for (int i = 0; i < n_int; ++i) {
-            const float dt = tg[i + 1] - tg[i];
-            const float* tp = ctx->t_grid + (size_t)i * S;
-            if (S == 2) {
-                if (eval_velocity(ctx, s, tp, 1, y0, B_img, yb, cfg_scale, k[0])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(0, y0, k[0], nullptr, nullptr, nullptr, 0.5f * dt, ytmp, n);
-                LAUNCH_OK();
-                if (eval_velocity(ctx, s, tp + 1, 1, ytmp, B_img, yb, cfg_scale, k[1])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(1, y0, nullptr, k[1], nullptr, nullptr, dt, y0, n);
-                LAUNCH_OK();
-            } else {
-                if (eval_velocity(ctx, s, tp, 1, y0, B_img, yb, cfg_scale, k[0])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(2, y0, k[0], nullptr, nullptr, nullptr, dt, ytmp, n);
-                LAUNCH_OK();
-                if (eval_velocity(ctx, s, tp + 1, 1, ytmp, B_img, yb, cfg_scale, k[1])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(3, y0, k[0], k[1], nullptr, nullptr, dt, ytmp, n);
-                LAUNCH_OK();
-                if (eval_velocity(ctx, s, tp + 2, 1, ytmp, B_img, yb, cfg_scale, k[2])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(4, y0, k[0], k[1], k[2], nullptr, dt, ytmp, n);
-                LAUNCH_OK();
-                if (eval_velocity(ctx, s, tp + 3, 1, ytmp, B_img, yb, cfg_scale, k[3])) return 1;
-                fixed_rk_stage_kernel<<<blocks_for(n), 256, 0, s>>>(5, y0, k[0], k[1], k[2], k[3], dt, y0, n);
-                LAUNCH_OK();
-            }
-            nfe += S;
-        }
-        CUDA_OK(cudaMemcpyAsync(x_inout, y0, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        if (join_out(ctx, user)) return 1;
-        if (stats != nullptr) {
-            stats->nfe = nfe;
-            stats->accepted = n_int;
-            stats->rejected = 0;
-        }
-        return 0;
-    }
-
-    // build (or fetch) the step graphs first: the warm-up run clobbers the solver state
-    cudaGraphExec_t g_euler = nullptr, g_heun = nullptr;
-    const int n_int = n_grid - 1;
-    const int n_heun = method == LFM_METHOD_HEUN ? (heun_corrector_limit < n_int ? (heun_corrector_limit < 0 ? 0 : heun_corrector_limit) : n_int) : 0;
     if (join_in(ctx, user)) return 1;
-    int l_euler = 0, l_heun = 0;
-    if (n_heun < n_int && get_step_graph(ctx, 0, B_img, has_y, cfg_scale, &g_euler, &l_euler)) return 1;
-    if (n_heun > 0 && get_step_graph(ctx, 1, B_img, has_y, cfg_scale, &g_heun, &l_heun)) return 1;
     cudaStream_t s = ctx->stream;
-    CUDA_OK(cudaMemcpyAsync(ctx->t_grid, t_grid_host, (size_t)n_grid * sizeof(float), cudaMemcpyDefault, s));
-    CUDA_OK(cudaMemcpyAsync(ctx->x_state, x_inout, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+
+    // The stage times of the whole trajectory, computed here in fp32 exactly as the Python expressions do
+    // (t0 + dt * (1/3) ...).  options["perturb"]: the first evaluation of a step one ulp past t0 (Perturb.NEXT), rk4's
+    // last one ulp before t1 (Perturb.PREV) - in torchdiffeq's negated time; here in model time the directions flip.
+    std::vector<float> tg(n_grid), ts((size_t)n_int * S);
+    cudaPointerAttributes pa{};
+    CUDA_OK(cudaPointerGetAttributes(&pa, t_grid_host));
+    if (pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged)
+        CUDA_OK(cudaMemcpy(tg.data(), t_grid_host, n_grid * sizeof(float), cudaMemcpyDeviceToHost));
+    else  // a host array is read directly: cudaMemcpy between two pageable buffers is a driver-staged copy
+        memcpy(tg.data(), t_grid_host, n_grid * sizeof(float));
+    const float third = (float)(1.0 / 3.0), two_thirds = (float)(2.0 / 3.0);
+    for (int i = 0; i < n_int; ++i) {
+        const float t0 = tg[i], t1 = tg[i + 1], dt = t1 - t0;
+        float* ti = &ts[(size_t)i * S];
+        ti[0] = perturb ? nextafterf(t0, t0 - 1.0f) : t0;
+        if (method == LFM_METHOD_HEUN) {
+            ti[1] = t1;
+        } else if (method == LFM_METHOD_MIDPOINT) {
+            ti[1] = t0 + 0.5f * dt;
+        } else if (method == LFM_METHOD_RK4) {
+            ti[1] = t0 + dt * third;
+            ti[2] = t0 + dt * two_thirds;
+            ti[3] = perturb ? nextafterf(t1, t1 + 1.0f) : t1;
+        }
+    }
+    CUDA_OK(cudaMemcpyAsync(ctx->t_grid, tg.data(), tg.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(ctx->t_stage, ts.data(), ts.size() * sizeof(float), cudaMemcpyHostToDevice, s));
     if (has_y) CUDA_OK(cudaMemcpyAsync(ctx->y_buf, y, (size_t)rows * sizeof(long long), cudaMemcpyDefault, s));
-    StepState st0{0, n_int, perturb};
-    CUDA_OK(cudaMemcpyAsync(ctx->step_state, &st0, sizeof(st0), cudaMemcpyHostToDevice, s));
-    CUDA_OK(cudaStreamSynchronize(s));  // st0 / t_grid_host are host stack/pageable memory
+
+    // The step graphs.  Heun's intervals past the corrector limit replay an Euler step on stage 0 of the Heun table.
+    // A new graph's warm-up run reads the step counter (reset first: the table index scales with S) and clobbers
+    // the counter and the state, which are initialised afterwards.
+    const int n_main = method == LFM_METHOD_HEUN ? std::min(std::max(heun_corrector_limit, 0), n_int) : n_int;
+    auto step_graph = [&](int m, lfm_ctx::StepGraph* g) {
+        char key[128];
+        snprintf(key, sizeof(key), "m%d_s%d_n%d_y%d_c%.6f", m, S, B_img, has_y ? 1 : 0, cfg_scale > 1.0f ? cfg_scale : 0.f);
+        return get_graph(ctx, key, [&] { return record_fixed_step(ctx, m, S, B_img, has_y, cfg_scale); }, g);
+    };
+    lfm_ctx::StepGraph g_main, g_tail;
+    CUDA_OK(cudaMemsetAsync(ctx->step_state, 0, sizeof(StepState), s));
+    if (n_main > 0 && step_graph(method, &g_main)) return 1;
+    if (n_main < n_int && step_graph(LFM_METHOD_EULER, &g_tail)) return 1;
+    CUDA_OK(cudaMemsetAsync(ctx->step_state, 0, sizeof(StepState), s));
+    CUDA_OK(cudaMemcpyAsync(ctx->x_state, x_inout, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaStreamSynchronize(s));  // tg / ts are pageable host memory
     int64_t nfe = 0;
     for (int i = 0; i < n_int; ++i) {
-        const int kind = i < n_heun ? 1 : 0;
-        CUDA_OK(cudaGraphLaunch(kind ? g_heun : g_euler, s));
-        ctx->launches += kind ? l_heun : l_euler;
-        nfe += kind ? 2 : 1;
+        const bool main_kind = i < n_main;
+        CUDA_OK(cudaGraphLaunch(main_kind ? g_main.exec : g_tail.exec, s));
+        ctx->launches += main_kind ? g_main.launches : g_tail.launches;
+        nfe += main_kind ? S : 1;
     }
     CUDA_OK(cudaMemcpyAsync(x_inout, ctx->x_state, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (join_out(ctx, user)) return 1;
@@ -1031,7 +996,6 @@ struct Dopri {
     size_t n;
     int64_t nfe = 0;
     RkTableau tab{};
-    int method = 0;
 };
 
 // k_out = -v(t = -s_time, y)   (model sees a 0-d fp32 time)
@@ -1040,7 +1004,7 @@ static int dp_func(Dopri& d, float s_time, const float* yv, float* k_out) {
     const float t = -s_time;
     set_scalar_kernel<<<1, 32, 0, d.s>>>(ctx->t_eval, t);  // by-value launch argument: no host synchronisation
     LAUNCH_OK();
-    if (eval_velocity(ctx, d.s, ctx->t_eval, 1, yv, d.n_img, d.y, d.cfg_scale, k_out)) return 1;
+    if (eval_velocity(ctx, d.s, ctx->t_eval, 1, yv, d.n_img, d.y, d.cfg_scale, 0, k_out)) return 1;
     negate_kernel<<<blocks_for(d.n), 256, 0, d.s>>>(k_out, d.n);
     LAUNCH_OK();
     d.nfe++;
@@ -1084,7 +1048,7 @@ static int dp_record_step(Dopri& d, float atol, float rtol) {
         float* yi = (i == ns - 1 && d.tab.fsal) ? y1 : ytmp;
         rk_combine_dev_kernel<<<blocks_for(n), 256, 0, s>>>(y0, kp, i + 1, ctx->dp_dev->coef[i], yi, n);
         LAUNCH_OK();
-        if (eval_velocity(ctx, s, ctx->dp_dev->t + i, 1, yi, d.n_img, d.y, d.cfg_scale, ctx->kbuf[i + 1])) return 1;
+        if (eval_velocity(ctx, s, ctx->dp_dev->t + i, 1, yi, d.n_img, d.y, d.cfg_scale, 0, ctx->kbuf[i + 1])) return 1;
         negate_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->kbuf[i + 1], n);
         LAUNCH_OK();
     }
@@ -1098,39 +1062,6 @@ static int dp_record_step(Dopri& d, float atol, float rtol) {
     rms_finalize_kernel<<<1, 32, 0, s>>>(ctx->partial, kRmsBlocks, n, ctx->ratio);
     LAUNCH_OK();
     CUDA_OK(cudaMemcpyAsync(ctx->ratio_host, ctx->ratio, sizeof(float), cudaMemcpyDeviceToHost, s));
-    return 0;
-}
-
-static int dp_get_graph(Dopri& d, float atol, float rtol, cudaGraphExec_t* out, int* launches) {
-    lfm_ctx* ctx = d.ctx;
-    char key[160];
-    snprintf(key, sizeof(key), "dp%d_n%d_y%d_c%.6f_a%.9g_r%.9g", d.method, d.n_img, d.y != nullptr ? 1 : 0,
-             d.cfg_scale > 1.0f ? d.cfg_scale : 0.f, atol, rtol);
-    auto it = ctx->graphs.find(key);
-    if (it != ctx->graphs.end()) {
-        *out = it->second.exec;
-        *launches = it->second.launches;
-        return 0;
-    }
-    // warm-up run outside of capture (lazily set function attributes); it only writes scratch: ytmp, y1, k2..k7, ratio
-    const int64_t before = ctx->launches;
-    if (dp_record_step(d, atol, rtol)) return 1;
-    CUDA_OK(cudaStreamSynchronize(d.s));
-    const int per = static_cast<int>(ctx->launches - before);
-    cudaGraph_t graph = nullptr;
-    CUDA_OK(cudaStreamBeginCapture(d.s, cudaStreamCaptureModeThreadLocal));
-    const int rc = dp_record_step(d, atol, rtol);
-    cudaError_t e = cudaStreamEndCapture(d.s, &graph);
-    ctx->launches = before;
-    if (rc) return 1;
-    if (e != cudaSuccess) return fail(ctx, "dopri5 graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t exec = nullptr;
-    CUDA_OK(cudaGraphInstantiate(&exec, graph, 0));
-    CUDA_OK(cudaGraphDestroy(graph));
-    ctx->graphs[key].exec = exec;
-    ctx->graphs[key].launches = per;
-    *out = exec;
-    *launches = per;
     return 0;
 }
 
@@ -1153,7 +1084,6 @@ extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, dou
     if (join_in(ctx, user)) return 1;
     Dopri d{ctx, ctx->stream, B_img, nullptr, cfg_scale, (size_t)B_img * ctx->chw};
     d.tab = make_tableau(method);
-    d.method = method;
     const RkTableau& tab = d.tab;
     const int ns = tab.n;
     cudaStream_t s = d.s;
@@ -1170,11 +1100,14 @@ extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, dou
     RkPtrs kp;
     for (int j = 0; j < 7; ++j) kp.k[j] = k[j];
 
-    // the step graph first: its warm-up run scribbles over the scratch buffers (never over y0 / k1, set below)
-    cudaGraphExec_t g_step = nullptr;
-    int l_step = 0;
+    // the step graph first: its warm-up run scribbles over the scratch buffers ytmp, y1, k2..k7 and ratio (never over
+    // y0 / k1, set below)
+    lfm_ctx::StepGraph g_step;
     CUDA_OK(cudaMemsetAsync(ctx->dp_dev, 0, sizeof(DpStep), s));
-    if (dp_get_graph(d, atol_f, rtol_f, &g_step, &l_step)) return 1;
+    char key[160];
+    snprintf(key, sizeof(key), "dp%d_n%d_y%d_c%.6f_a%.9g_r%.9g", method, B_img, d.y != nullptr ? 1 : 0,
+             cfg_scale > 1.0f ? cfg_scale : 0.f, atol_f, rtol_f);
+    if (get_graph(ctx, key, [&] { return dp_record_step(d, atol_f, rtol_f); }, &g_step)) return 1;
 
     CUDA_OK(cudaMemcpyAsync(y0, x_inout, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
     double s0 = -t0;
@@ -1218,8 +1151,8 @@ extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, dou
             for (int j = 0; j <= ns; ++j) hp->coef[ns][j] = (float)tab.c_sol[j] * dt_32;
         for (int j = 0; j <= ns; ++j) hp->cerr[j] = dt_32 * (float)tab.c_err[j];
         CUDA_OK(cudaMemcpyAsync(ctx->dp_dev, hp, sizeof(DpStep), cudaMemcpyHostToDevice, s));
-        CUDA_OK(cudaGraphLaunch(g_step, s));
-        ctx->launches += l_step;
+        CUDA_OK(cudaGraphLaunch(g_step.exec, s));
+        ctx->launches += g_step.launches;
         CUDA_OK(cudaStreamSynchronize(s));  // the ONE synchronisation of the step: the controller runs on the host in fp64
         d.nfe += ns;
         const float ratio = fabsf(ctx->ratio_host[0]);

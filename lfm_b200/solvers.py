@@ -67,7 +67,9 @@ def _check_labels(net, y, rows, device):
     return y
 
 
-def _run_fixed(model, x, y, cfg_scale, t_nodes, method, t_as_vector, corrector_limit):
+def _run_native(model, x, y, cfg_scale, entry, method, *args):
+    """Integrate a float32 copy of x with the native sampler ``entry`` (lfm_sample_fixed or lfm_sample_adaptive), called
+    as ``entry(ctx, method, x, *args, y, B_img, cfg_scale, stats, stream)``.  Returns (x_final, stats dict)."""
     net = _unwrap(model)
     if not x.is_cuda:
         raise RuntimeError("lfm_b200 solvers run on CUDA tensors only")
@@ -76,14 +78,18 @@ def _run_fixed(model, x, y, cfg_scale, t_nodes, method, t_as_vector, corrector_l
     rows = 2 * n_img if cfg_scale > 1.0 else n_img
     y = _check_labels(net, y, rows, x.device)
     ctx = net.native(rows, x.device)
-    grid = t_nodes.detach().to("cpu", torch.float32).contiguous()
     stats = _lib.OdeStats()
-    _lib.check(_lib.load().lfm_sample_fixed(
-        ctx, {"euler": 0, "heun": 1, "midpoint": 2, "rk4": 3}[method], x.data_ptr(), grid.data_ptr(), grid.numel(), int(t_as_vector),
-        int(corrector_limit), y.data_ptr() if y is not None else None, n_img, float(cfg_scale), C.byref(stats),
+    _lib.check(getattr(_lib.load(), entry)(
+        ctx, method, x.data_ptr(), *args, y.data_ptr() if y is not None else None, n_img, float(cfg_scale), C.byref(stats),
         _NativeNet._stream(x.device)), ctx)
     net.last_stats = dict(nfe=int(stats.nfe), accepted=int(stats.accepted), rejected=int(stats.rejected))
     return x, net.last_stats
+
+
+def _run_fixed(model, x, y, cfg_scale, t_nodes, method, t_as_vector, corrector_limit):
+    grid = t_nodes.detach().to("cpu", torch.float32).contiguous()
+    return _run_native(model, x, y, cfg_scale, "lfm_sample_fixed", {"euler": 0, "heun": 1, "midpoint": 2, "rk4": 3}[method],
+                       grid.data_ptr(), grid.numel(), int(t_as_vector), int(corrector_limit))
 
 
 def euler_time_grid(step_size: float, t0: float = 1.0, t1: float = 0.0) -> torch.Tensor:
@@ -114,18 +120,8 @@ def sample_from_model(model, x_0, model_kwargs, args):
         nodes = euler_time_grid(float(args.step_size))
         xf, stats = _run_fixed(model, x, y, cfg_scale, nodes, method, flags, 0)
     elif method in ("dopri5", "bosh3", "adaptive_heun"):
-        net = _unwrap(model)
-        xf = x.to(torch.float32).contiguous().clone()
-        n_img = xf.shape[0]
-        rows = 2 * n_img if cfg_scale > 1.0 else n_img
-        y = _check_labels(net, y, rows, xf.device)
-        ctx = net.native(rows, xf.device)
-        st = _lib.OdeStats()
-        _lib.check(_lib.load().lfm_sample_adaptive(ctx, {"dopri5": 0, "bosh3": 1, "adaptive_heun": 2}[method], xf.data_ptr(), 1.0, 0.0,
-                                                   float(args.rtol), float(args.atol), y.data_ptr() if y is not None else None,
-                                                   n_img, float(cfg_scale), C.byref(st), _NativeNet._stream(xf.device)), ctx)
-        stats = dict(nfe=int(st.nfe), accepted=int(st.accepted), rejected=int(st.rejected))
-        net.last_stats = stats
+        xf, stats = _run_native(model, x, y, cfg_scale, "lfm_sample_adaptive", {"dopri5": 0, "bosh3": 1, "adaptive_heun": 2}[method],
+                                1.0, 0.0, float(args.rtol), float(args.atol))
     else:
         raise NotImplementedError(f"method '{method}' has no native implementation (euler, midpoint, rk4, dopri5, bosh3 and "
                                   "adaptive_heun do)")

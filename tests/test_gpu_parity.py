@@ -294,6 +294,12 @@ def test_dopri5_with_cfg_vs_oracle(dev):
     # accept/reject decisions can flip by one step under bf16 noise in v; the solution must still agree
     assert abs(net.last_stats["nfe"] - st.nfe) <= 6 and net.last_stats["nfe"] == 2 + 6 * (
         net.last_stats["accepted"] + net.last_stats["rejected"])
+    # fixed-grid rk4 with labels and CFG: four stage times per step from the step graph's table
+    args = types.SimpleNamespace(method="rk4", step_size=0.2, perturb=False, cfg_scale=1.5, compute_nfe=True)
+    traj, nfe = lfm_b200.sample_from_model(net, torch.cat([x, x]).to(dev), dict(y=y2.to(dev), cfg_scale=1.5), args)
+    ref, n = osol.tdq_fixed_rk(oracle_model(sd, cfg, y2, 1.5), torch.cat([x, x]), 0.2, "rk4")
+    assert int(nfe) == n == 20 and torch.equal(traj[-1][:2], traj[-1][2:])
+    assert rel_l2(traj[-1].cpu(), ref) < TOL_E2E
 
 
 # ------------------------------------------------------------------------------------------------ full-size properties
