@@ -195,10 +195,43 @@ int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void
 /* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer in the timm feature order ({q,k,v} * D + head * 64 + c) -> out [B*256, D]
  * bf16.  variant 0: the TMA + wgmma kernel the network runs for 256 tokens; 1: the mma.sync flash kernel.  dbg_s must be NULL. */
 int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s, void* stream);
-/* The mma.sync attention kernels of the DiT geometries (16 / 64 tokens: whole sequence in registers;
- * other multiples of 64, e.g. 256 / 1024: keys streamed in chunks of 64).  qkv [B*T, 3*H*ch] bf16 with HEAD-MAJOR features
- * (head * 3 ch + {q,k,v} * ch + c), ch = 64 or 80 (head_dim 72 zero-padded), scale head_dim^-1/2 -> out [B*T, H*ch] bf16. */
+/* The mma.sync attention kernels (16 / 64 tokens: whole sequence in registers, ch = 64, 80, 128 or 256; other multiples of 64,
+ * e.g. 256 / 1024: keys streamed in chunks of 64, ch = 64 or 80).  qkv [B*T, 3*H*ch] bf16 with HEAD-MAJOR features
+ * (head * 3 ch + {q,k,v} * ch + c) -> out [B*T, H*ch] bf16.  Scale head_dim^-1/2 (DiT-XL: ch = 80 is head_dim 72 zero-padded);
+ * head_dim 0: ch^-1/2, on 16 / 64 tokens computed by the kernel itself as in the UNets. */
 int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream);
+/* The UNet programs' 3x3 convolution (pad 1) as the implicit GEMM the network runs, built and launched by the network's own code.
+ *   x: bf16 NHWC [B, side, side, Cin] (Cin % 64 == 0); stride 1 or 2 (output side side / stride: 4, 8, ..., 256).
+ *   w: bf16 [Cout, 9 Cin], K index (r * 3 + s) * Cin + c (lfm_set_param's repacked order); bias: fp32 [Cout]; Cout 4 or % 8 == 0.
+ *   out: [B, side/stride, side/stride, Cout]: epi 3 fp32 = conv + bias, 0 bf16 = conv + bias, 2 fp32 out += conv + bias.
+ *   block_n: 0 = the network's tile width for the shape, or 128 / 256.
+ *   ksplit: -1 = the network's split-K decision for B images, 1 = none, 2..8 = that many K slices (epi 3 / 2, block_n 0 / 128).
+ *   gn_bins: NULL, or the GroupNorm statistics of the output taken in the epilogue (u64 [B][16 replicas][32 groups][sum, sum of
+ *   squares], the sum in units of 2^-28 and the sum of squares in 2^-20; accumulated: the caller zeroes it).  Needs epi 3 / 0, no
+ *   split-K, Cout / 32 in {4, 8, 16, 32, 64} and a multiple of 32 output pixels.
+ * The entry allocates its own split-K scratch on `stream`. */
+int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
+                 int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
+/* The batched GEMM of the VAE mid-block attention: M = B * out_hw rows in groups of batch_m; group g computes
+ * out[g rows] = A[rows] W[g * b_batch_rows .. + N]^T (+ bias), A row = row % a_mod when a_mod > 0 (A shared by all groups).
+ * a: bf16 [a_rows, K] with row pitch a_ld, w: bf16 [w_rows, K] with row pitch w_ld (column windows of wider matrices);
+ * out [M, N] fp32 (epi 3) or bf16 (epi 0); bias fp32 [N] or NULL.  K % 64 == 0, N % 256 == 0, batch_m % 128 == 0. */
+int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w_bf16, int w_rows, int w_ld, int K, int N, void* out,
+                         const float* bias, int B, int out_hw, int epi, int batch_m, int a_mod, int b_batch_rows, void* stream);
+/* The UNet programs' GroupNorm(32 groups) pass over B images of HW pixels, with the network's launch code.
+ *   source: the channel concatenation [a (Ca channels) | b (Cb channels)] of fp32 NHWC tensors (b NULL when Cb = 0), C = Ca + Cb
+ *   a multiple of 128 up to 2048; src_bf16: NULL, or the same values as bf16 [B, HW, C] to read instead.
+ *   bins: NULL = the statistics pass over the fp32 source, in at most max_chunks pixel chunks per image (32 in the UNets, 256 in
+ *   the VAE); else the statistics as lfm_dbg_conv's gn_bins.
+ *   out = act(((x - mean) * rstd * gamma + beta) * (1 + film[c]) + film[C + c]): gamma, beta fp32 [C]; film NULL or fp32 rows
+ *   [scale (C) | shift (C)] at film + b * film_stride; act 1 = SiLU; eps > 0.
+ *   out bf16 [B, HW, C]; copy_out: NULL or fp32 [B, HW, C] = the source; raw_out: NULL or bf16 [B, HW, C] = the source as bf16. */
+int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb, const void* src_bf16, const unsigned long long* bins,
+                      int max_chunks, const float* gamma, const float* beta, const float* film, int film_stride, int act, float eps,
+                      void* out_bf16, float* copy_out, void* raw_out, int B, int HW, void* stream);
+/* The UNet programs' attention (QKVAttentionLegacy): qkv bf16 [B*T, 3C], HEAD-MAJOR (head * 3 ch + {q,k,v} * ch + c, ch = C / heads)
+ * -> out bf16 [B*T, C], softmax(q k^T / sqrt(ch)) v, on the kernel the network picks for (T, ch).  Shapes no kernel covers are refused. */
+int lfm_dbg_unet_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int C, int heads, void* stream);
 /* Intermediate activations of the last lfm_forward (fp32 token stream [B*T, D] after all blocks). */
 int lfm_dbg_tokens(lfm_ctx* ctx, float* out, int B);
 

@@ -1267,20 +1267,171 @@ extern "C" int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, in
 
 extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream) {
     lfm_ctx* ctx = nullptr;
+    if (!(ch == 64 || ch == 80 || ch == 128 || ch == 256) || head_dim < 0 || head_dim > ch)
+        return fail(ctx, "lfm_dbg_attention_mma: ch must be 64, 80, 128 or 256 and 0 <= head_dim <= ch (got ch %d, head_dim %d)", ch, head_dim);
+    const bool short_grid = T == 16 || T == 64;
+    if (!short_grid && !(T > 0 && T % 64 == 0 && (ch == 64 || ch == 80)))
+        return fail(ctx, "lfm_dbg_attention_mma: T must be 16 or 64, or a multiple of 64 with ch 64 / 80 (got T %d, ch %d)", T, ch);
+    if (B < 1 || H < 1) return fail(ctx, "lfm_dbg_attention_mma: B and H must be >= 1 (got %d, %d)", B, H);
     g_num_sms = query_num_sms();
     if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    if (!(ch == 64 || ch == 80) || head_dim <= 0 || head_dim > ch) return fail(ctx, "lfm_dbg_attention_mma: ch must be 64 or 80, head_dim <= ch");
-    const float sc = 1.4426950408889634f / sqrtf(static_cast<float>(head_dim));
+    // head_dim 0: the short-grid kernel's own ch^-1/2 (what the UNets run); the flash kernel always takes the scale from the host
+    const float sc = head_dim > 0 ? 1.4426950408889634f / sqrtf(static_cast<float>(head_dim))
+                                  : (short_grid ? 0.f : 1.4426950408889634f / sqrtf(static_cast<float>(ch)));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv_bf16);
     __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out_bf16);
-    if (T == 16 || T == 64)
+    if (short_grid)
         CUDA_OK(launch_attention_mma(s, q, o, T, ch, H * ch, H, B * H, sc));
-    else if (T > 0 && T % 64 == 0)
-        CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
     else
-        return fail(ctx, "lfm_dbg_attention_mma: T must be 16 or a multiple of 64 (got %d)", T);
+        CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
     return 0;
+}
+
+// The entries below run one op of the UNet program through the program's own construction (push_*) and launch (run_*_op)
+// helpers.  `dbg` stands in for the network context: it receives the error message and counts the launches.
+static bool conv_out_side_ok(int s) { return s == 4 || s == 8 || s == 16 || s == 32 || s == 64 || s == 128 || s == 256; }
+
+extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B,
+                            int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
+    lfm_ctx* ctx = nullptr;
+    if (B < 1) return fail(ctx, "lfm_dbg_conv: B must be >= 1 (got %d)", B);
+    if (stride != 1 && stride != 2) return fail(ctx, "lfm_dbg_conv: stride must be 1 or 2 (got %d)", stride);
+    if (side % stride != 0 || !conv_out_side_ok(side / stride))
+        return fail(ctx, "lfm_dbg_conv: side %d with stride %d: the output side must be 4, 8, 16, 32, 64, 128 or 256", side, stride);
+    if (Cin < 64 || Cin % 64 != 0) return fail(ctx, "lfm_dbg_conv: Cin must be a positive multiple of 64 (got %d)", Cin);
+    if (!(Cout == 4 || (Cout >= 8 && Cout % 8 == 0))) return fail(ctx, "lfm_dbg_conv: Cout must be 4 or a multiple of 8 (got %d)", Cout);
+    if (block_n != 0 && block_n != 128 && block_n != 256)
+        return fail(ctx, "lfm_dbg_conv: block_n must be 0, 128 or 256 (got %d)", block_n);
+    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16 && epi != EPI_GATE_RESID_F32)
+        return fail(ctx, "lfm_dbg_conv: epi must be 3 (fp32 out), 0 (bf16 out) or 2 (out += conv) (got %d)", epi);
+    if (ksplit != -1 && (ksplit < 1 || ksplit > 8))
+        return fail(ctx, "lfm_dbg_conv: ksplit must be -1 (the network's plan), 1 (none) or 2..8 (got %d)", ksplit);
+    if (ksplit > 1 && (epi == EPI_BIAS_BF16 || block_n == 256))
+        return fail(ctx, "lfm_dbg_conv: ksplit %d: split-K writes fp32 (epi 3 or 2) with 128-wide tiles (block_n 0 or 128)", ksplit);
+    const int out_hw = (side / stride) * (side / stride), cpg = Cout / 32;
+    if (gn_bins != nullptr && (epi == EPI_GATE_RESID_F32 || ksplit > 1 || Cout % 32 != 0 ||
+                               !(cpg == 4 || cpg == 8 || cpg == 16 || cpg == 32 || cpg == 64) || out_hw % 32 != 0))
+        return fail(ctx, "lfm_dbg_conv: gn_bins needs epi 3 or 0, no split-K, Cout / 32 in {4, 8, 16, 32, 64} and a multiple of 32 "
+                         "output pixels (got epi %d, ksplit %d, Cout %d, %d pixels)", epi, ksplit, Cout, out_hw);
+    if (x_bf16 == nullptr || w_bf16 == nullptr || bias == nullptr || out == nullptr)
+        return fail(ctx, "lfm_dbg_conv: x, w, bias and out must not be NULL");
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+    lfm_ctx dbg;
+    ctx = &dbg;
+    UNetState u;
+    if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16), bias,
+                   Cout, out, epi))
+        return fail(ctx, "lfm_dbg_conv: tensor map encode failed");
+    UOp& o = u.prog[0];
+    if (ksplit >= 1) {
+        o.ksplit = ksplit;
+        o.split_pitch = ksplit > 1 ? (B * out_hw + kGemmBlockM - 1) / kGemmBlockM * kGemmBlockM : 0;
+    }
+    if (o.ksplit > 1 && (block_n == 256 || gn_bins != nullptr))
+        return fail(ctx, "lfm_dbg_conv: the network splits K %d ways here: pass ksplit 1 for block_n 256 or gn_bins", o.ksplit);
+    if (gn_bins != nullptr) {
+        o.bins_slot = 0;
+        u.BINS = gn_bins;
+        u.bins_rows = B;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (o.ksplit > 1) CUDA_OK(cudaMallocAsync(&u.SPLIT, (size_t)o.ksplit * o.split_pitch * o.N * sizeof(float), s));
+    const int rc = run_gemm_op(ctx, &u, o, s, B, block_n);
+    if (u.SPLIT != nullptr) CUDA_OK(cudaFreeAsync(u.SPLIT, s));
+    return rc;
+}
+
+extern "C" int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w_bf16, int w_rows, int w_ld, int K, int N,
+                                    void* out, const float* bias, int B, int out_hw, int epi, int batch_m, int a_mod, int b_batch_rows,
+                                    void* stream) {
+    lfm_ctx* ctx = nullptr;
+    if (K < 64 || K % 64 != 0 || N < 256 || N % 256 != 0)
+        return fail(ctx, "lfm_dbg_gemm_batched: K must be a multiple of 64 and N of 256 (got K %d, N %d)", K, N);
+    if (a_rows < 1 || w_rows < 1 || a_ld < K || w_ld < K || a_ld % 8 != 0 || w_ld % 8 != 0)
+        return fail(ctx, "lfm_dbg_gemm_batched: a_ld / w_ld must be >= K and multiples of 8, a_rows / w_rows >= 1 "
+                         "(got a %d x ld %d, w %d x ld %d)", a_rows, a_ld, w_rows, w_ld);
+    if (batch_m < 128 || batch_m % 128 != 0 || a_mod < 0 || a_mod % 128 != 0 || b_batch_rows < N)
+        return fail(ctx, "lfm_dbg_gemm_batched: batch_m must be a positive multiple of 128, a_mod 0 or a multiple of 128, "
+                         "b_batch_rows >= N (got batch_m %d, a_mod %d, b_batch_rows %d)", batch_m, a_mod, b_batch_rows);
+    if (B < 1 || out_hw < 1 || ((long long)B * out_hw) % batch_m != 0)
+        return fail(ctx, "lfm_dbg_gemm_batched: B * out_hw must be a positive multiple of batch_m (got %d x %d)", B, out_hw);
+    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16) return fail(ctx, "lfm_dbg_gemm_batched: epi must be 3 (fp32) or 0 (bf16) (got %d)", epi);
+    if (a_bf16 == nullptr || w_bf16 == nullptr || out == nullptr) return fail(ctx, "lfm_dbg_gemm_batched: a, w and out must not be NULL");
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+    lfm_ctx dbg;
+    ctx = &dbg;
+    UNetState u;
+    if (!push_batched(&u, a_bf16, a_rows, a_ld, K, w_bf16, w_rows, w_ld, N, out, out_hw, epi, bias, batch_m, a_mod, b_batch_rows))
+        return fail(ctx, "lfm_dbg_gemm_batched: tensor map encode failed");
+    return run_gemm_op(ctx, &u, u.prog[0], static_cast<cudaStream_t>(stream), B, 0);
+}
+
+extern "C" int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb, const void* src_bf16, const unsigned long long* bins,
+                                 int max_chunks, const float* gamma, const float* beta, const float* film, int film_stride, int act,
+                                 float eps, void* out_bf16, float* copy_out, void* raw_out, int B, int HW, void* stream) {
+    lfm_ctx* ctx = nullptr;
+    const int C = Ca + Cb;
+    if (Ca < 4 || Ca % 4 != 0 || Cb < 0 || Cb % 4 != 0 || (b == nullptr) != (Cb == 0))
+        return fail(ctx, "lfm_dbg_groupnorm: Ca must be a positive multiple of 4, Cb 0 (b NULL) or a multiple of 4 (got %d, %d)", Ca, Cb);
+    if (C % 128 != 0 || C > 128 * kGnMaxJ) return fail(ctx, "lfm_dbg_groupnorm: Ca + Cb must be a multiple of 128 up to %d (got %d)", 128 * kGnMaxJ, C);
+    if (B < 1 || B > 65535 || HW < 1) return fail(ctx, "lfm_dbg_groupnorm: B must be in [1, 65535] and HW >= 1 (got %d, %d)", B, HW);
+    if (bins == nullptr && (max_chunks < 1 || max_chunks > 256))
+        return fail(ctx, "lfm_dbg_groupnorm: max_chunks must be in [1, 256] (got %d)", max_chunks);
+    if (act != 0 && act != 1) return fail(ctx, "lfm_dbg_groupnorm: act must be 0 or 1 (SiLU) (got %d)", act);
+    if (film_stride < 0 || !(eps > 0.f)) return fail(ctx, "lfm_dbg_groupnorm: film_stride must be >= 0 and eps > 0");
+    if (a == nullptr || gamma == nullptr || beta == nullptr || out_bf16 == nullptr)
+        return fail(ctx, "lfm_dbg_groupnorm: a, gamma, beta and out must not be NULL");
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+    lfm_ctx dbg;
+    ctx = &dbg;
+    UNetState u;
+    u.gn_eps = eps;
+    u.max_chunks = max_chunks;
+    push_gn(&u, Src2{a, b, Ca, Cb}, HW, C, gamma, beta, film != nullptr ? 0 : -1, act, static_cast<__nv_bfloat16*>(out_bf16), copy_out,
+            static_cast<__nv_bfloat16*>(raw_out));
+    u.film = const_cast<float*>(film);
+    UOp& st = u.prog[0];
+    UOp& ap = u.prog[1];
+    ap.gn_src_bf16 = static_cast<const __nv_bfloat16*>(src_bf16);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (bins != nullptr) {  // statistics from a producing convolution's epilogue: [B][kGnBinReplicas][32 groups][sum, sum of squares]
+        st.skip = true;
+        ap.bins_slot = 0;
+        u.BINS = const_cast<unsigned long long*>(bins);
+        u.bins_rows = B;
+    } else {
+        CUDA_OK(cudaMallocAsync(&u.partial, (size_t)B * max_chunks * 64 * sizeof(double), s));
+    }
+    int rc = 0;
+    for (const UOp& o : u.prog)
+        if (rc == 0 && !o.skip) rc = run_gn_op(ctx, &u, o, s, B, film_stride);
+    if (u.partial != nullptr) CUDA_OK(cudaFreeAsync(u.partial, s));
+    return rc;
+}
+
+extern "C" int lfm_dbg_unet_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int C, int heads, void* stream) {
+    lfm_ctx* ctx = nullptr;
+    if (B < 1 || heads < 1 || C % heads != 0)
+        return fail(ctx, "lfm_dbg_unet_attention: B and heads must be >= 1 and C a multiple of heads (got B %d, C %d, heads %d)", B, C, heads);
+    if (!unet_attn_supported(T, C / heads))
+        return fail(ctx, "lfm_dbg_unet_attention: %d tokens with a head width of %d channels is not supported", T, C / heads);
+    if (qkv_bf16 == nullptr || out_bf16 == nullptr) return fail(ctx, "lfm_dbg_unet_attention: qkv and out must not be NULL");
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+    lfm_ctx dbg;
+    ctx = &dbg;
+    UOp o;
+    o.kind = U_ATTN;
+    o.qkv = static_cast<const __nv_bfloat16*>(qkv_bf16);
+    o.att = static_cast<__nv_bfloat16*>(out_bf16);
+    o.HW = T;
+    o.C = C;
+    o.heads = heads;
+    return run_attn_op(ctx, o, static_cast<cudaStream_t>(stream), B);
 }
 
 extern "C" int lfm_dbg_tokens(lfm_ctx* ctx, float* out, int B) {

@@ -114,8 +114,8 @@ LFM_DEVICE void gn_coefficients(const GnApplyArgs& a, int b, float* s_coef, floa
                 si += static_cast<long long>(bp[0]);
                 qi += static_cast<long long>(bp[1]);
             }
-            S = static_cast<double>(si) / 268435456.0;
-            Q = static_cast<double>(qi) / 268435456.0;
+            S = static_cast<double>(si) / kGnFixScale;
+            Q = static_cast<double>(qi) / kGnFixScaleSq;
         } else {
             for (int c = 0; c < a.nchunk; ++c) {  // fixed order => deterministic
                 S += a.partial[(static_cast<size_t>(b) * a.nchunk + c) * 64 + 2 * threadIdx.x];

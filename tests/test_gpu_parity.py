@@ -9,6 +9,7 @@ the stored qkv / attention / MLP-hidden activations to bf16:
   * end-to-end sampler output vs the fp32 reference fixture ....... rel-L2 <= 2e-3   (measured ~3e-5)
   * solver arithmetic given identical velocities .................. bit-exact / <= 1e-6
   * kernel-level GEMM vs fp32 matmul of the same bf16 operands .... fp32 out <= 1e-5, bf16 out <= 4e-3 (1 bf16 ulp)
+The UNet / EDM / VAE kernels are compared op by op in tests/test_gpu_kernels.py.
 """
 import ctypes as C
 import types
@@ -72,9 +73,13 @@ def make_big(model_type, dev, num_classes, label_dropout, max_batch):
     (256, 256, 64, 3, 0), (768, 1152, 384, 0, 0), (512, 1024, 4096, 2, 0), (16384, 1024, 4096, 2, 0),
     (16384, 3072, 1024, 1, 0), (768, 768, 384, 1, 0), (16384, 3072, 1024, 0, 0), (512, 256, 64, 3, 0), (256, 256, 128, 3, 0),
     (1280, 768, 256, 1, 0), (4096, 1024, 1024, 2, 0), (16384, 4096, 1024, 0, 0), (32768, 1024, 1024, 2, 0),
-    (38 * 512, 512, 128, 3, 0)])
+    (38 * 512, 512, 128, 3, 0),
+    # "resid": the residual epilogue with gate NULL (out += acc + bias), every UNet conv2 and attention projection
+    (4096, 256, 2304, "resid", 0), (1024, 1024, 4608, "resid", 256), (2048, 512, 512, "resid", 128), (300, 8, 64, "resid", 0)])
 def test_gemm_epilogues(dev, M, N, K, epi, bn):
     lib = _lib.load()
+    gated = epi != "resid"
+    epi = epi if gated else 2
     g = torch.Generator().manual_seed(M + N + K + epi)
     a = (torch.randn(M, K, generator=g) * 0.5).to(dev).bfloat16()
     w = (torch.randn(N, K, generator=g) * 0.05).to(dev).bfloat16()
@@ -90,12 +95,12 @@ def test_gemm_epilogues(dev, M, N, K, epi, bn):
     elif epi == 2:
         x0 = torch.randn(M, N, generator=g).to(dev)
         out = x0.clone()
-        ref = x0 + gate[torch.arange(M, device=dev) // Tt, N:2 * N] * acc
+        ref = x0 + (gate[torch.arange(M, device=dev) // Tt, N:2 * N] * acc if gated else acc)
         tol = 1e-5
     else:
         out, ref, tol = torch.zeros(M, N, device=dev), acc, 1e-5
-    rc = lib.lfm_dbg_gemm(P(a), P(w), P(bias), P(out), C.c_void_p(gate.data_ptr() + N * 4), 3 * N, Tt, M, N, K, epi, bn,
-                          None)
+    gate_p = C.c_void_p(gate.data_ptr() + N * 4) if gated else None
+    rc = lib.lfm_dbg_gemm(P(a), P(w), P(bias), P(out), gate_p, 3 * N, Tt, M, N, K, epi, bn, None)
     torch.cuda.synchronize()
     assert rc == 0, _lib.last_error()
     assert rel_l2(out.float().cpu(), ref.cpu()) < tol

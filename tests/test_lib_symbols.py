@@ -67,3 +67,117 @@ def test_unsupported_shapes_are_rejected(lib):
     # GEMM tile widths are 128 and 256 (0: the network's pick); anything else is refused before the device is touched
     assert lib.lfm_dbg_gemm(None, None, None, None, None, 0, 1, 128, 128, 64, 3, 640, None) != 0
     assert "block_n" in _lib.last_error()
+
+
+def test_kernel_entries_refuse_bad_arguments(lib):
+    """Every kernel-level entry checks its shape arguments before it touches the device, and names the bad argument."""
+    from lfm_b200 import _lib
+
+    def refused(rc, word):
+        assert rc != 0
+        assert word in _lib.last_error(), _lib.last_error()
+
+    # lfm_dbg_conv(x, w, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream)
+    conv = lib.lfm_dbg_conv
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 640, 3, -1, None), "block_n")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 3, 0, 3, -1, None), "stride")
+    refused(conv(None, None, None, None, None, 1, 2, 128, 128, 1, 0, 3, -1, None), "side")
+    refused(conv(None, None, None, None, None, 1, 512, 128, 128, 1, 0, 3, -1, None), "side")
+    refused(conv(None, None, None, None, None, 1, 32, 96, 128, 1, 0, 3, -1, None), "Cin")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 12, 1, 0, 3, -1, None), "Cout")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 0, 1, -1, None), "epi")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 0, 3, 9, None), "ksplit")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 0, 0, 2, None), "ksplit")
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 256, 3, 4, None), "ksplit")
+    refused(conv(None, None, None, None, None, 0, 32, 128, 128, 1, 0, 3, -1, None), "B")
+    dummy = ctypes.c_void_p(64)   # never dereferenced: each call below is refused on its shape arguments
+    refused(conv(None, None, None, None, dummy, 1, 32, 128, 128, 1, 0, 2, 1, None), "gn_bins")     # residual epilogue
+    refused(conv(None, None, None, None, dummy, 1, 32, 128, 96, 1, 0, 3, 1, None), "gn_bins")      # 3 channels per group
+    refused(conv(None, None, None, None, dummy, 1, 4, 128, 128, 1, 0, 3, 1, None), "gn_bins")      # 16 output pixels
+    refused(conv(None, None, None, None, None, 1, 32, 128, 128, 1, 0, 3, -1, None), "NULL")
+    # lfm_dbg_gemm_batched(a, a_rows, a_ld, w, w_rows, w_ld, K, N, out, bias, B, out_hw, epi, batch_m, a_mod, b_batch_rows, stream)
+    bat = lib.lfm_dbg_gemm_batched
+    refused(bat(None, 256, 512, None, 256, 512, 512, 128, None, None, 1, 256, 3, 256, 0, 256, None), "N")
+    refused(bat(None, 256, 512, None, 256, 512, 96, 256, None, None, 1, 256, 3, 256, 0, 256, None), "K")
+    refused(bat(None, 256, 256, None, 256, 512, 512, 256, None, None, 1, 256, 3, 256, 0, 256, None), "a_ld")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 256, 3, 200, 0, 256, None), "batch_m")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 256, 3, 256, 64, 256, None), "a_mod")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 256, 3, 256, 0, 128, None), "b_batch_rows")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 384, 3, 256, 0, 256, None), "batch_m")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 256, 2, 256, 0, 256, None), "epi")
+    refused(bat(None, 256, 512, None, 256, 512, 512, 256, None, None, 1, 256, 3, 256, 0, 256, None), "NULL")
+    # lfm_dbg_groupnorm(a, Ca, b, Cb, src_bf16, bins, max_chunks, gamma, beta, film, film_stride, act, eps, out, copy_out, raw_out,
+    #                   B, HW, stream)
+    gn = lib.lfm_dbg_groupnorm
+    refused(gn(None, 200, None, 0, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "Ca + Cb")
+    refused(gn(None, 2048, dummy, 256, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "Ca + Cb")
+    refused(gn(None, 256, None, 512, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "Cb")
+    refused(gn(None, 256, None, 0, None, None, 0, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "max_chunks")
+    refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 2, 1e-5, None, None, None, 1, 64, None), "act")
+    refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 0.0, None, None, None, 1, 64, None), "eps")
+    refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 0, 64, None), "B")
+    refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "NULL")
+    # lfm_dbg_unet_attention(qkv, out, B, T, C, heads, stream): the shapes no UNet attention kernel covers (see below)
+    att = lib.lfm_dbg_unet_attention
+    refused(att(None, None, 1, 1024, 128, 1, None), "1024 tokens")
+    refused(att(None, None, 1, 64, 384, 1, None), "384 channels")
+    refused(att(None, None, 1, 64, 384, 32, None), "12 channels")
+    refused(att(None, None, 1, 64, 128, 3, None), "heads")
+    refused(att(None, None, 1, 64, 128, 2, None), "NULL")
+    # lfm_dbg_attention_mma(qkv, out, B, H, T, ch, head_dim, stream)
+    mma = lib.lfm_dbg_attention_mma
+    refused(mma(None, None, 1, 1, 64, 96, 0, None), "ch")
+    refused(mma(None, None, 1, 1, 64, 64, 72, None), "head_dim")
+    refused(mma(None, None, 1, 1, 256, 128, 0, None), "T")
+    refused(mma(None, None, 1, 1, 48, 64, 64, None), "T")
+
+
+def _unet_desc(cfg):
+    from lfm_b200 import _lib
+    ar, cm = cfg.attention_resolutions, cfg.channel_mult
+    return _lib.UnetDesc(cfg.image_size, cfg.in_channels, cfg.model_channels, cfg.out_channels, cfg.num_res_blocks, len(ar),
+                         (ctypes.c_int32 * 8)(*ar), len(cm), (ctypes.c_int32 * 8)(*cm), cfg.num_heads, cfg.num_head_channels,
+                         cfg.num_classes or 0)
+
+
+@pytest.mark.parametrize("kw,words", [
+    # 32 x 32 = 1024 tokens with one 128-channel head (in the input, output and middle blocks)
+    (dict(image_size=32, model_channels=128, channel_mult=(1, 2), attention_resolutions=(1,), num_heads=1), ("1024 tokens", "128")),
+    # the middle block alone: 8 x 8 = 64 tokens with one 384-channel head
+    (dict(image_size=8, model_channels=384, channel_mult=(1,), attention_resolutions=(), num_heads=1), ("64 tokens", "384")),
+    # 12-channel heads (16-byte loads need multiples of 8)
+    (dict(image_size=8, model_channels=384, channel_mult=(1,), attention_resolutions=(), num_heads=32), ("64 tokens", "12 channels")),
+    # 128 channels do not split into 3 heads
+    (dict(image_size=8, model_channels=128, channel_mult=(1,), attention_resolutions=(), num_heads=3), ("128 channels", "3 heads")),
+    (dict(image_size=8, model_channels=128, channel_mult=(1,), attention_resolutions=(), num_heads=1, num_head_channels=0),
+     ("num_head_channels",)),
+])
+def test_unet_attention_shapes_without_a_kernel_are_refused(lib, kw, words):
+    """UNetModel shapes whose attention no kernel covers are refused by the constructor, before it looks for a device."""
+    from lfm_b200 import _lib
+    from oracle import unet as ounet
+    ctx = ctypes.c_void_p()
+    assert lib.lfm_create_unet(ctypes.byref(_unet_desc(ounet.UNetConfig(**kw))), 0, ctypes.byref(ctx)) != 0
+    msg = _lib.last_error()
+    assert "lfm_create_unet" in msg and "device" not in msg, msg
+    for w in words:
+        assert w in msg, msg
+
+
+def test_fixture_unet_configurations_pass_the_attention_check(lib):
+    """Every UNetModel configuration the tests and the benchmark build gets past the attention check: without a GPU the
+    constructor then fails on the missing device; with one it succeeds."""
+    from lfm_b200 import _lib
+    from oracle import unet as ounet
+    from tests._util import load_golden
+    from tests.test_oracle_unet import unet_cfg_from_golden
+    cfgs = [unet_cfg_from_golden(load_golden("unet_mini")), unet_cfg_from_golden(load_golden("unet_mini_cond")),
+            ounet.UNetConfig(image_size=32, channel_mult=(1, 2, 2, 2)),   # celeb256
+            ounet.UNetConfig()]                                           # celeb512 (BASELINE cfg4)
+    for cfg in cfgs:
+        ctx = ctypes.c_void_p()
+        rc = lib.lfm_create_unet(ctypes.byref(_unet_desc(cfg)), 0, ctypes.byref(ctx))
+        if rc == 0:
+            lib.lfm_destroy(ctx)
+        else:
+            assert "device" in _lib.last_error(), (cfg, _lib.last_error())
