@@ -87,7 +87,7 @@ typedef struct lfm_edm_desc {
  * latent_channels 4, out_channels 3).  diffusers is a third-party dependency outside /root/reference: the architecture
  * is restated in oracle/vae.py (parity unpinned). */
 typedef struct lfm_vae_desc {
-    int32_t latent_size;            /* latent side = image_size // 8: 16, 32 (256 x 256 images; the LFM presets) */
+    int32_t latent_size;            /* latent side = image_size // 8: 16, 32 or 64 (128, 256, 512 pixel images) */
     int32_t latent_channels;        /* 4 */
     int32_t out_channels;           /* 3 */
     int32_t n_blocks;               /* number of entries used in block_out_channels */
@@ -212,6 +212,11 @@ int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, in
  * The entry allocates its own split-K scratch on `stream`. */
 int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
                  int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
+/* The same convolution for output rows wider than one 128-pixel tile (the VAE decoder's 256- and 512-pixel stages, run on
+ * 128-pixel row segments): side 256 or 512, stride 1, ksplit 1 (never split along K); x, w, bias, out, gn_bins, block_n and epi as
+ * lfm_dbg_conv.  Arguments are checked before the device is touched. */
+int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
+                      int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
 /* The batched GEMM of the VAE mid-block attention: M = B * out_hw rows in groups of batch_m; group g computes
  * out[g rows] = A[rows] W[g * b_batch_rows .. + N]^T (+ bias), A row = row % a_mod when a_mod > 0 (A shared by all groups).
  * a: bf16 [a_rows, K] with row pitch a_ld, w: bf16 [w_rows, K] with row pitch w_ld (column windows of wider matrices);

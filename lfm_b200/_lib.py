@@ -62,6 +62,7 @@ SYMBOLS = {
     "lfm_dbg_attention": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "lfm_dbg_attention_mma": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_conv_wide": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_gemm_batched": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int,
                                        C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_groupnorm": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P,

@@ -360,7 +360,7 @@ def main(argv=None):
         return 0
 
     # default: one batch; every rank samples (and decodes) its shard and ONE all-gather assembles the result on all
-    # ranks - of the decoded uint8 images when the native decoder runs (196 KB per 256 x 256 image), else of the latents
+    # ranks - of the decoded uint8 images when the native decoder runs (196 KB per 256 x 256 image, 768 KB at 512), else of the latents
     out = run_sampling(args.batch_size, generator, as_uint8=True)
     out = ldist.all_gather_batch(out)
     if rank == 0:

@@ -31,7 +31,8 @@ struct GemmEpi {
     // bins[((row / gn_hw) * kGnBinReplicas + r) * 64 + 2 g + {0,1}] += {sum, sum of squares} of group g = column / gn_cpg, as
     // fixed point: the sum in units of 2^-28, the sum of squares in units of 2^-20 (integer atomics => the result does not depend
     // on the order of arrival: deterministic).  The signed 64-bit totals hold |sum| < 2^35 and a sum of squares < 2^43 ~ 8.8e12 per
-    // (image, group): rms 5793 at the VAE's 256 x 256 x 128 stage (2^18 values per group), 16384 at a 64 x 64 x 256 UNet layer.
+    // (image, group): rms 2896 at the 512-pixel VAE decode's 512 x 512 x 128 stage (2^20 values per group), 5793 at the
+    // 256-pixel decode's 256 x 256 x 128 stage (2^18), 16384 at a 64 x 64 x 256 UNet layer.
     // Each add rounds to half a unit, so at rms 1e-2 the sum of squares of the VAE stage (26.2, from 4096 adds per group) is off by
     // at most 2e-3, 7e-5 relative.  r is any of
     // kGnBinReplicas copies (chosen per warp; the consumer adds them up - integers, so still exact), so that the atomics of
@@ -49,8 +50,10 @@ constexpr double kGnFixScaleSq = 1048576.0;  // 2^20: the sum of squares
 
 // Implicit-GEMM convolution geometry (taps == 0: plain GEMM, A is a 2-D [M, K] matrix).
 // Output pixels are flattened (b, h, w) row-major; a tile's 128 output rows are whole image rows (W * rows == 128),
-// whole images (H * W divides 128) or one 128-pixel segment of an image row (W = 256: the VAE decoder's last stage),
-// so the matching input window of tap (r, s) is ONE 4-D box.
+// whole images (H * W divides 128) or one 128-pixel segment of an image row (W a multiple of 128: the VAE decoder's last
+// stages, W = 256 or 512; make_tmap_act4d refuses any other W above 128), so the matching input window of tap (r, s) is ONE
+// 4-D box.  A segment's box starts at w0 - 1 and ends at w0 + 128: the columns left of 0 and right of W - 1 are the TMA's
+// zero fill (the padding), the ones across an inner seam are the neighbouring segment's pixels.
 struct ConvGeom {
     int taps;     // 0 (GEMM), 9 (3x3, pad 1)
     int cblocks;  // C_in / 64
@@ -247,7 +250,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 if (cg.taps != 0) {
                     img0 = row_a / cg.HW;
                     h0 = (row_a % cg.HW) / cg.W;
-                    w0 = row_a % cg.W;  // non-zero only when an image row is wider than the 128-pixel tile (W = 256)
+                    w0 = row_a % cg.W;  // non-zero only when an image row is wider than the 128-pixel tile (W = 256, 512)
                 }
                 const int kb0 = ks * kb_per, kb1 = min(num_kb, kb0 + kb_per);
                 int tap = 0, cb = 0;

@@ -1290,6 +1290,39 @@ extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B
 
 // The entries below run one op of the UNet program through the program's own construction (push_*) and launch (run_*_op)
 // helpers.  `dbg` stands in for the network context: it receives the error message and counts the launches.
+// The device half of lfm_dbg_conv / lfm_dbg_conv_wide, on checked arguments.  ksplit -1 keeps push_conv's plan.
+static int dbg_conv_launch(const char* who, const void* x_bf16, const void* w_bf16, const float* bias, void* out,
+                           unsigned long long* gn_bins, int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit,
+                           void* stream) {
+    lfm_ctx* ctx = nullptr;
+    const int out_hw = (side / stride) * (side / stride);
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+    lfm_ctx dbg;
+    ctx = &dbg;
+    UNetState u;
+    if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16), bias,
+                   Cout, out, epi))
+        return fail(ctx, "%s: tensor map encode failed", who);
+    UOp& o = u.prog[0];
+    if (ksplit >= 1) {
+        o.ksplit = ksplit;
+        o.split_pitch = ksplit > 1 ? (B * out_hw + kGemmBlockM - 1) / kGemmBlockM * kGemmBlockM : 0;
+    }
+    if (o.ksplit > 1 && (block_n == 256 || gn_bins != nullptr))
+        return fail(ctx, "%s: the network splits K %d ways here: pass ksplit 1 for block_n 256 or gn_bins", who, o.ksplit);
+    if (gn_bins != nullptr) {
+        o.bins_slot = 0;
+        u.BINS = gn_bins;
+        u.bins_rows = B;
+    }
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (o.ksplit > 1) CUDA_OK(cudaMallocAsync(&u.SPLIT, (size_t)o.ksplit * o.split_pitch * o.N * sizeof(float), s));
+    const int rc = run_gemm_op(ctx, &u, o, s, B, block_n);
+    if (u.SPLIT != nullptr) CUDA_OK(cudaFreeAsync(u.SPLIT, s));
+    return rc;
+}
+
 static bool conv_out_side_ok(int s) { return s == 4 || s == 8 || s == 16 || s == 32 || s == 64 || s == 128 || s == 256; }
 
 extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B,
@@ -1316,31 +1349,31 @@ extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float*
                          "output pixels (got epi %d, ksplit %d, Cout %d, %d pixels)", epi, ksplit, Cout, out_hw);
     if (x_bf16 == nullptr || w_bf16 == nullptr || bias == nullptr || out == nullptr)
         return fail(ctx, "lfm_dbg_conv: x, w, bias and out must not be NULL");
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    lfm_ctx dbg;
-    ctx = &dbg;
-    UNetState u;
-    if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16), bias,
-                   Cout, out, epi))
-        return fail(ctx, "lfm_dbg_conv: tensor map encode failed");
-    UOp& o = u.prog[0];
-    if (ksplit >= 1) {
-        o.ksplit = ksplit;
-        o.split_pitch = ksplit > 1 ? (B * out_hw + kGemmBlockM - 1) / kGemmBlockM * kGemmBlockM : 0;
-    }
-    if (o.ksplit > 1 && (block_n == 256 || gn_bins != nullptr))
-        return fail(ctx, "lfm_dbg_conv: the network splits K %d ways here: pass ksplit 1 for block_n 256 or gn_bins", o.ksplit);
-    if (gn_bins != nullptr) {
-        o.bins_slot = 0;
-        u.BINS = gn_bins;
-        u.bins_rows = B;
-    }
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (o.ksplit > 1) CUDA_OK(cudaMallocAsync(&u.SPLIT, (size_t)o.ksplit * o.split_pitch * o.N * sizeof(float), s));
-    const int rc = run_gemm_op(ctx, &u, o, s, B, block_n);
-    if (u.SPLIT != nullptr) CUDA_OK(cudaFreeAsync(u.SPLIT, s));
-    return rc;
+    return dbg_conv_launch("lfm_dbg_conv", x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream);
+}
+
+// Stride-1 3x3 convolutions whose output rows are wider than one 128-pixel tile (the row-segment tiles of the VAE decoder's
+// last stages): the same push_conv / run_gemm_op path, never split along K.
+extern "C" int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins,
+                                 int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
+    lfm_ctx* ctx = nullptr;
+    if (side != 256 && side != 512) return fail(ctx, "lfm_dbg_conv_wide: side must be 256 or 512 (got %d)", side);
+    if (stride != 1) return fail(ctx, "lfm_dbg_conv_wide: stride must be 1 (got %d)", stride);
+    if (B < 1 || (long long)B * side * side > INT32_MAX)
+        return fail(ctx, "lfm_dbg_conv_wide: B must be >= 1 and B * side^2 below 2^31 output pixels (got B %d)", B);
+    if (Cin < 64 || Cin % 64 != 0) return fail(ctx, "lfm_dbg_conv_wide: Cin must be a positive multiple of 64 (got %d)", Cin);
+    if (!(Cout == 4 || (Cout >= 8 && Cout % 8 == 0))) return fail(ctx, "lfm_dbg_conv_wide: Cout must be 4 or a multiple of 8 (got %d)", Cout);
+    if (block_n != 0 && block_n != 128 && block_n != 256)
+        return fail(ctx, "lfm_dbg_conv_wide: block_n must be 0, 128 or 256 (got %d)", block_n);
+    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16 && epi != EPI_GATE_RESID_F32)
+        return fail(ctx, "lfm_dbg_conv_wide: epi must be 3 (fp32 out), 0 (bf16 out) or 2 (out += conv) (got %d)", epi);
+    if (ksplit != 1) return fail(ctx, "lfm_dbg_conv_wide: ksplit must be 1: wide rows are never split along K (got %d)", ksplit);
+    const int cpg = Cout / 32;
+    if (gn_bins != nullptr && (epi == EPI_GATE_RESID_F32 || Cout % 32 != 0 || !(cpg == 4 || cpg == 8 || cpg == 16 || cpg == 32 || cpg == 64)))
+        return fail(ctx, "lfm_dbg_conv_wide: gn_bins needs epi 3 or 0 and Cout / 32 in {4, 8, 16, 32, 64} (got epi %d, Cout %d)", epi, Cout);
+    if (x_bf16 == nullptr || w_bf16 == nullptr || bias == nullptr || out == nullptr)
+        return fail(ctx, "lfm_dbg_conv_wide: x, w, bias and out must not be NULL");
+    return dbg_conv_launch("lfm_dbg_conv_wide", x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, 1, block_n, epi, 1, stream);
 }
 
 extern "C" int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w_bf16, int w_rows, int w_ld, int K, int N,

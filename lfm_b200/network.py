@@ -92,6 +92,10 @@ class _NativeNet(nn.Module):
     def _create_ctx(self, lib, dev_index):  # -> ctypes handle
         raise NotImplementedError
 
+    def _finalize_rows(self, rows: int) -> int:
+        """Rows the native workspace is sized for when a context is (re)created for `rows`."""
+        return max(rows, self.max_batch_hint or 0)
+
     def native(self, rows: int, device: torch.device):
         """Return the lfm_ctx handle, (re)creating it and uploading the weights when needed."""
         lib = _lib.load()
@@ -114,7 +118,7 @@ class _NativeNet(nn.Module):
                 t = p.detach().to(torch.float32).contiguous()
                 shape = (C.c_int64 * t.dim())(*t.shape)
                 _lib.check(lib.lfm_set_param(ctx, key.encode(), C.c_void_p(t.data_ptr()), 0, shape, t.dim()), ctx)
-            max_rows = max(rows, self.max_batch_hint or 0)
+            max_rows = self._finalize_rows(rows)
             _lib.check(lib.lfm_finalize(ctx, max_rows), ctx)
         except Exception:
             lib.lfm_destroy(ctx)

@@ -163,7 +163,7 @@ class AutoencoderKL(_NativeNet):
         up = 2 ** (len(self.block_out_channels) - 1)
         out = torch.empty(B, self.out_channels, h * up, w * up, device=z.device) if want_f32 else None
         u8 = torch.empty(B, h * up, w * up, self.out_channels, device=z.device, dtype=torch.uint8) if want_u8 else None
-        chunk = max(1, int(self.max_batch_hint or 16))
+        chunk = self.decode_chunk(h)
         ctx = self.native(min(B, chunk), z.device)
         lib = _lib.load()
         for i in range(0, B, chunk):
@@ -171,6 +171,16 @@ class AutoencoderKL(_NativeNet):
             _lib.check(lib.lfm_decode(ctx, z[i:i + n].data_ptr(), n, out[i:i + n].data_ptr() if want_f32 else None,
                                       u8[i:i + n].data_ptr() if want_u8 else None, self._stream(z.device)), ctx)
         return out, u8
+
+    def decode_chunk(self, latent_side: int) -> int:
+        """Images per native decode call, and the batch the native workspace is sized for: ``max_batch`` (default 16) for
+        latents up to 32 x 32.  A 512 x 512 image (64 x 64 latents) needs four times the workspace of a 256 x 256 one, about
+        1.2 GB per image, so there the chunk is ``max_batch // 4``: the same bytes as the 256-pixel decode at the same hint."""
+        hint = max(1, int(self.max_batch_hint or 16))
+        return max(1, hint // 4) if latent_side >= 64 else hint
+
+    def _finalize_rows(self, rows):
+        return max(rows, self.decode_chunk(self._latent_size))
 
     # -- first_stage_model.decode(z).sample  (test_flow_latent.py:193) --------------------------------------------------
     def decode(self, z, return_dict=True, **kwargs):
