@@ -57,18 +57,22 @@ static EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// Row-major bf16 matrix [rows, cols]; box = 64 columns (one 128-byte swizzle row) x box_rows rows.
-static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// Row-major bf16 matrix [rows, cols] with a row pitch of ld elements (ld > cols: a column window of a wider matrix);
+// box = 64 columns (one 128-byte swizzle row) x box_rows rows.
+static bool make_tmap_bf16_ld(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
     EncodeTiledFn fn = get_encode_fn();
     if (fn == nullptr) return false;
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 2};
+    cuuint64_t strides[1] = {ld * 2};
     cuuint32_t box[2] = {64, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
+}
+static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    return make_tmap_bf16_ld(m, base, rows, cols, cols, box_rows);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -196,19 +200,31 @@ static inline unsigned blocks_for(size_t n, int threads = 256) { return static_c
 // ------------------------------------------------------------------------------------------------
 // context
 
+// What lfm_set_param makes of an fp32 source.  Every transform but F32 reads the source from the staging buffer.
+enum class Xform {
+    F32,              // plain fp32 copy
+    BF16,             // cast to bf16
+    CONV_BF16,        // conv weight [Co, Ci, kh, kw] -> bf16 [Co, kh, kw, Ci]
+    TRANSPOSE_F32,    // fp32 [R, rest] -> [rest, R]
+    EDM_QKV_W,        // EDM qkv weight / bias rows re-ordered (aux0 = head dim, aux1 = target layout, edm_qkv_src_row)
+    EDM_QKV_B,
+    RESAMPLE_FILTER,  // the constant resample_filter of EDM.py:96-98: validated, not stored
+    DIT_QKV_W,        // DiT qkv weight / bias rows re-ordered head-major for the mma.sync attention kernels
+    DIT_QKV_B,        //   (aux0 = head dim, aux1 = its stored, zero-padded width)
+    DIT_PROJ_PAD,     // DiT proj weight with zero columns for the padded head channels (aux0, aux1 as above)
+};
+
 struct ParamSlot {
     void* dst = nullptr;        // device destination (fp32 or bf16)
     std::vector<int64_t> shape;
     size_t numel = 0;
-    bool to_bf16 = false;
-    int kind = 0;  // 0 copy fp32, 1 cast bf16, 2 conv [Co,Ci,kh,kw] -> bf16 [Co,kh,kw,Ci], 3 out-conv -> fp32 [4][9][C],
-                   // 4 fp32 transpose [R, rest] -> [rest, R], 5 / 6 EDM qkv weight / bias row re-order (aux0 = head dim,
-                   // aux1 = target layout), 7 constant resample_filter (validated, not stored), 8 / 9 DiT qkv weight / bias rows
-                   // re-ordered head-major for the mma.sync attention kernels (aux0 = head dim, aux1 = its stored, zero-padded width),
-                   // 10 DiT proj weight with zero columns for the padded head channels
+    Xform xform = Xform::F32;
     int aux0 = 0, aux1 = 0;
     bool set = false;
 };
+
+// The network a context runs: lfm_create's DiT, or one of the three flavours of the UNet program (unet_host.inc, ctx->un).
+enum class NetKind { DIT, ADM, EDM, VAE };
 
 struct BlockW {
     __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;
@@ -220,7 +236,7 @@ struct UNetState;
 
 struct lfm_ctx {
     lfm_model_desc d{};
-    int arch = LFM_ARCH_DIT;
+    NetKind net = NetKind::DIT;
     UNetState* un = nullptr;
     int device = 0;
     int num_sms = 0;
@@ -290,25 +306,131 @@ static int dev_alloc(lfm_ctx* ctx, Tp** p, size_t count) {
     return 0;
 }
 
-static void add_param(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, bool to_bf16) {
-    ParamSlot s;
-    s.dst = dst;
-    s.shape = shape;
-    s.numel = 1;
-    for (int64_t v : shape) s.numel *= static_cast<size_t>(v);
-    s.to_bf16 = to_bf16;
-    s.kind = to_bf16 ? 1 : 0;
-    ctx->params[key] = s;
-}
-static void add_param_kind(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, int kind) {
-    add_param(ctx, key, dst, shape, kind != 0);
-    ctx->params[key].kind = kind;
+static size_t numel(const std::vector<int64_t>& shape) {
+    size_t n = 1;
+    for (int64_t v : shape) n *= static_cast<size_t>(v);
+    return n;
 }
 
-static void add_param_aux(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, int kind, int aux0, int aux1) {
-    add_param_kind(ctx, key, dst, shape, kind);
-    ctx->params[key].aux0 = aux0;
-    ctx->params[key].aux1 = aux1;
+static void add_param(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, Xform xform = Xform::F32,
+                      int aux0 = 0, int aux1 = 0) {
+    ParamSlot s;
+    s.dst = dst;
+    s.numel = numel(shape);
+    s.shape = std::move(shape);
+    s.xform = xform;
+    s.aux0 = aux0;
+    s.aux1 = aux1;
+    ctx->params[key] = s;
+}
+
+// A parameter whose storage holds exactly its registered shape: allocate numel(shape) elements and register them.
+template <typename Tp>
+static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::vector<int64_t>& shape, Xform xform = Xform::F32,
+                       int aux0 = 0, int aux1 = 0) {
+    if (dev_alloc(ctx, p, numel(shape))) return 1;
+    add_param(ctx, key, *p, shape, xform, aux0, aux1);
+    return 0;
+}
+
+// Makes the context's device current and gives the launch helpers its SM count: the first step of every entry that uses the device.
+static int bind(lfm_ctx* ctx) {
+    CUDA_OK(cudaSetDevice(ctx->device));
+    g_num_sms = ctx->num_sms;
+    return 0;
+}
+
+// A context of `kind` on `device`, with its stream and both events.  The creators call it after their own shape checks, so a
+// shape refusal never depends on the device.
+static int new_ctx(const char* who, int device, NetKind kind, lfm_ctx** out) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+        return fail(nullptr, "%s: no CUDA device (liblfm_b200 has no CPU path)", who);
+    if (device < 0 || device >= ndev) return fail(nullptr, "%s: bad device %d", who, device);
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
+    if (prop.major != 9) return fail(nullptr, "%s: device %d is sm_%d%d; this library is sm_90a only", who, device, prop.major, prop.minor);
+    lfm_ctx* ctx = new lfm_ctx();
+    ctx->net = kind;
+    ctx->device = device;
+    ctx->num_sms = prop.multiProcessorCount;
+    auto init = [&]() -> int {
+        if (bind(ctx)) return 1;
+        CUDA_OK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
+        CUDA_OK(cudaEventCreateWithFlags(&ctx->ev_in, cudaEventDisableTiming));
+        CUDA_OK(cudaEventCreateWithFlags(&ctx->ev_out, cudaEventDisableTiming));
+        return 0;
+    };
+    if (init()) {
+        lfm_destroy(ctx);
+        return 1;
+    }
+    *out = ctx;
+    return 0;
+}
+
+// The creators' last step: hand out the context, or release it when building it failed (rc != 0).  The message stays
+// available through lfm_last_error(NULL).
+static int finish_create(lfm_ctx* ctx, int rc, lfm_ctx** out) {
+    if (rc) {
+        lfm_destroy(ctx);
+        return 1;
+    }
+    *out = ctx;
+    return 0;
+}
+
+// DiT parameter storage and state-dict keys.
+static int dit_register(lfm_ctx* ctx) {
+    const lfm_model_desc& d = ctx->d;
+    const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T, Dq = ctx->Dq;
+    const int ps = d.patch_size;
+    const int P = ctx->C * ps * ps;  // elements of one patch = out-features of the final linear
+    if (alloc_param(ctx, "pos_embed", &ctx->pos, {1, T, D}) ||
+        alloc_param(ctx, "x_embedder.proj.weight", &ctx->pe_w, {D, 4, ps, ps}, Xform::TRANSPOSE_F32) ||  // stored as [P, D]
+        alloc_param(ctx, "x_embedder.proj.bias", &ctx->pe_b, {D}) ||
+        alloc_param(ctx, "t_embedder.mlp.0.weight", &ctx->t_w0, {D, 256}) ||
+        alloc_param(ctx, "t_embedder.mlp.0.bias", &ctx->t_b0, {D}) ||
+        alloc_param(ctx, "t_embedder.mlp.2.weight", &ctx->t_w2, {D, D}) ||
+        alloc_param(ctx, "t_embedder.mlp.2.bias", &ctx->t_b2, {D}) ||
+        alloc_param(ctx, "y_embedder.embedding_table.weight", &ctx->ytable, {d.table_rows, D}) ||
+        alloc_param(ctx, "final_layer.linear.weight", &ctx->fin_w, {P, D}) ||
+        alloc_param(ctx, "final_layer.linear.bias", &ctx->fin_b, {P}))
+        return 1;
+    // all adaLN modulation layers in one table: block i at rows 6 i D, the final layer's after them
+    if (dev_alloc(ctx, &ctx->w_mod, (size_t)ctx->Nmod * D)) return 1;
+    if (dev_alloc(ctx, &ctx->b_mod, ctx->Nmod)) return 1;
+    add_param(ctx, "final_layer.adaLN_modulation.1.weight", ctx->w_mod + (size_t)6 * L * D * D, {2 * D, D}, Xform::BF16);
+    add_param(ctx, "final_layer.adaLN_modulation.1.bias", ctx->b_mod + (size_t)6 * L * D, {2 * D});
+    ctx->blk.resize(L);
+    for (int i = 0; i < L; ++i) {
+        BlockW& b = ctx->blk[i];
+        const std::string p = "blocks." + std::to_string(i) + ".";
+        // qkv and proj are stored with the padded head width dhp (Dq = H * dhp columns of attention output)
+        if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
+        if (dev_alloc(ctx, &b.b_qkv, 3 * Dq)) return 1;
+        if (dev_alloc(ctx, &b.w_proj, (size_t)D * Dq)) return 1;
+        if (ctx->qkv_head_major) {
+            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::DIT_QKV_W, ctx->dh, ctx->dhp);
+            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, Xform::DIT_QKV_B, ctx->dh, ctx->dhp);
+        } else {
+            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::BF16);
+            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D});
+        }
+        if (ctx->dhp != ctx->dh)
+            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::DIT_PROJ_PAD, ctx->dh, ctx->dhp);
+        else
+            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::BF16);
+        if (alloc_param(ctx, p + "attn.proj.bias", &b.b_proj, {D}) ||
+            alloc_param(ctx, p + "mlp.fc1.weight", &b.w_fc1, {Hd, D}, Xform::BF16) ||
+            alloc_param(ctx, p + "mlp.fc1.bias", &b.b_fc1, {Hd}) ||
+            alloc_param(ctx, p + "mlp.fc2.weight", &b.w_fc2, {D, Hd}, Xform::BF16) ||
+            alloc_param(ctx, p + "mlp.fc2.bias", &b.b_fc2, {D}))
+            return 1;
+        add_param(ctx, p + "adaLN_modulation.1.weight", ctx->w_mod + (size_t)i * 6 * D * D, {6 * D, D}, Xform::BF16);
+        add_param(ctx, p + "adaLN_modulation.1.bias", ctx->b_mod + (size_t)i * 6 * D, {6 * D});
+    }
+    return 0;
 }
 
 extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out) {
@@ -334,18 +456,8 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
         return fail(nullptr, "lfm_create: head_dim must be 64 or 72 (hidden %d, heads %d)", desc->hidden_size, desc->num_heads);
     if (desc->mlp_hidden % 64 != 0) return fail(nullptr, "lfm_create: mlp_hidden must be a multiple of 64");
     if (desc->in_channels != 4) return fail(nullptr, "lfm_create: in_channels must be 4");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail(nullptr, "lfm_create: no CUDA device (liblfm_b200 has no CPU path)");
-    if (device < 0 || device >= ndev) return fail(nullptr, "lfm_create: bad device %d", device);
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
-    if (prop.major != 9) return fail(nullptr, "lfm_create: device %d is sm_%d%d; this library is sm_90a only", device, prop.major, prop.minor);
-    ctx = new lfm_ctx();
+    if (new_ctx("lfm_create", device, NetKind::DIT, &ctx)) return 1;
     ctx->d = *desc;
-    ctx->device = device;
-    CUDA_OK(cudaSetDevice(device));
-    g_num_sms = ctx->num_sms = prop.multiProcessorCount;
     ctx->D = desc->hidden_size;
     ctx->L = desc->depth;
     ctx->H = desc->num_heads;
@@ -356,78 +468,13 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->HW = desc->img_resolution;
     ctx->chw = ctx->C * ctx->HW * ctx->HW;
     ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
-    const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T;
-    const int ps = desc->patch_size;
-    const int P = ctx->C * ps * ps;  // elements of one patch = out-features of the final linear
     // 256 tokens with head_dim 64 (every released preset) keep the checkpoint's timm qkv order, which the flash kernel reads directly.
     // Everything else - 16 / 64 / 1024 tokens, head_dim 72 (DiT-XL, stored padded to 80) - stores the qkv rows head-major.
     ctx->dh = desc->hidden_size / desc->num_heads;
     ctx->dhp = ctx->dh == 72 ? 80 : 64;
     ctx->Dq = desc->num_heads * ctx->dhp;
-    ctx->qkv_head_major = (T != 256 || ctx->dh != 64);
-    const bool qkv_head_major = ctx->qkv_head_major;
-    const int Dq = ctx->Dq;
-
-    if (dev_alloc(ctx, &ctx->pos, (size_t)T * D)) return 1;
-    if (dev_alloc(ctx, &ctx->pe_w, (size_t)D * P)) return 1;
-    if (dev_alloc(ctx, &ctx->pe_b, D)) return 1;
-    if (dev_alloc(ctx, &ctx->t_w0, (size_t)D * 256)) return 1;
-    if (dev_alloc(ctx, &ctx->t_b0, D)) return 1;
-    if (dev_alloc(ctx, &ctx->t_w2, (size_t)D * D)) return 1;
-    if (dev_alloc(ctx, &ctx->t_b2, D)) return 1;
-    if (dev_alloc(ctx, &ctx->ytable, (size_t)desc->table_rows * D)) return 1;
-    if (dev_alloc(ctx, &ctx->fin_w, (size_t)P * D)) return 1;
-    if (dev_alloc(ctx, &ctx->fin_b, P)) return 1;
-    if (dev_alloc(ctx, &ctx->w_mod, (size_t)ctx->Nmod * D)) return 1;
-    if (dev_alloc(ctx, &ctx->b_mod, ctx->Nmod)) return 1;
-    add_param(ctx, "pos_embed", ctx->pos, {1, T, D}, false);
-    add_param_kind(ctx, "x_embedder.proj.weight", ctx->pe_w, {D, 4, ps, ps}, 4);  // stored transposed [P, D]
-    add_param(ctx, "x_embedder.proj.bias", ctx->pe_b, {D}, false);
-    add_param(ctx, "t_embedder.mlp.0.weight", ctx->t_w0, {D, 256}, false);
-    add_param(ctx, "t_embedder.mlp.0.bias", ctx->t_b0, {D}, false);
-    add_param(ctx, "t_embedder.mlp.2.weight", ctx->t_w2, {D, D}, false);
-    add_param(ctx, "t_embedder.mlp.2.bias", ctx->t_b2, {D}, false);
-    add_param(ctx, "y_embedder.embedding_table.weight", ctx->ytable, {desc->table_rows, D}, false);
-    add_param(ctx, "final_layer.linear.weight", ctx->fin_w, {P, D}, false);
-    add_param(ctx, "final_layer.linear.bias", ctx->fin_b, {P}, false);
-    add_param(ctx, "final_layer.adaLN_modulation.1.weight", ctx->w_mod + (size_t)6 * L * D * D, {2 * D, D}, true);
-    add_param(ctx, "final_layer.adaLN_modulation.1.bias", ctx->b_mod + (size_t)6 * L * D, {2 * D}, false);
-    ctx->blk.resize(L);
-    for (int i = 0; i < L; ++i) {
-        BlockW& b = ctx->blk[i];
-        if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
-        if (dev_alloc(ctx, &b.w_proj, (size_t)D * Dq)) return 1;
-        if (dev_alloc(ctx, &b.w_fc1, (size_t)Hd * D)) return 1;
-        if (dev_alloc(ctx, &b.w_fc2, (size_t)D * Hd)) return 1;
-        if (dev_alloc(ctx, &b.b_qkv, 3 * Dq)) return 1;
-        if (dev_alloc(ctx, &b.b_proj, D)) return 1;
-        if (dev_alloc(ctx, &b.b_fc1, Hd)) return 1;
-        if (dev_alloc(ctx, &b.b_fc2, D)) return 1;
-        const std::string p = "blocks." + std::to_string(i) + ".";
-        if (qkv_head_major) {
-            add_param_aux(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, 8, ctx->dh, ctx->dhp);
-            add_param_aux(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, 9, ctx->dh, ctx->dhp);
-        } else {
-            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, true);
-            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, false);
-        }
-        if (ctx->dhp != ctx->dh)
-            add_param_aux(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, 10, ctx->dh, ctx->dhp);  // zero columns for the padded channels
-        else
-            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, true);
-        add_param(ctx, p + "attn.proj.bias", b.b_proj, {D}, false);
-        add_param(ctx, p + "mlp.fc1.weight", b.w_fc1, {Hd, D}, true);
-        add_param(ctx, p + "mlp.fc1.bias", b.b_fc1, {Hd}, false);
-        add_param(ctx, p + "mlp.fc2.weight", b.w_fc2, {D, Hd}, true);
-        add_param(ctx, p + "mlp.fc2.bias", b.b_fc2, {D}, false);
-        add_param(ctx, p + "adaLN_modulation.1.weight", ctx->w_mod + (size_t)i * 6 * D * D, {6 * D, D}, true);
-        add_param(ctx, p + "adaLN_modulation.1.bias", ctx->b_mod + (size_t)i * 6 * D, {6 * D}, false);
-    }
-    CUDA_OK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-    CUDA_OK(cudaEventCreateWithFlags(&ctx->ev_in, cudaEventDisableTiming));
-    CUDA_OK(cudaEventCreateWithFlags(&ctx->ev_out, cudaEventDisableTiming));
-    *out = ctx;
-    return 0;
+    ctx->qkv_head_major = (ctx->T != 256 || ctx->dh != 64);
+    return finish_create(ctx, dit_register(ctx), out);
 }
 
 extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int dtype, const int64_t* shape, int ndim) {
@@ -440,9 +487,8 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
     for (int i = 0; i < ndim; ++i)
         if (shape[i] != s.shape[i])
             return fail(ctx, "lfm_set_param(%s): dim %d is %lld, expected %lld", key, i, (long long)shape[i], (long long)s.shape[i]);
-    CUDA_OK(cudaSetDevice(ctx->device));
-    g_num_sms = ctx->num_sms;
-    if (!s.to_bf16) {
+    if (bind(ctx)) return 1;
+    if (s.xform == Xform::F32) {
         CUDA_OK(cudaMemcpy(s.dst, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
     } else {
         if (ctx->staging_elems < s.numel) {
@@ -452,42 +498,57 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
             ctx->staging_elems = s.numel;
         }
         CUDA_OK(cudaMemcpy(ctx->staging, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
-        if (s.kind == 2) {
-            const int taps = static_cast<int>(s.shape[2] * s.shape[3]);
-            conv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
-                                                                   static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), taps);
-        } else if (s.kind == 4) {
-            const int r0 = static_cast<int>(s.shape[0]);
-            transpose_f32_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst), r0,
-                                                              static_cast<int>(s.numel / r0));
-        } else if (s.kind == 3) {
-            conv_out_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst),
-                                                                       static_cast<int>(s.shape[1]));
-        } else if (s.kind == 5) {
-            edm_qkv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
-                                                                      static_cast<int>(s.shape[1]), s.aux0, s.aux1);
-        } else if (s.kind == 6) {
-            edm_qkv_bias_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst),
-                                                                    static_cast<int>(s.shape[0] / 3), s.aux0, s.aux1);
-        } else if (s.kind == 8) {  // aux0 = head_dim, aux1 = stored head width: the destination has 3 * heads * aux1 rows
-            const int Dm = static_cast<int>(s.shape[1]);
-            const size_t out_n = static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1 * Dm;
-            dit_qkv_weight_repack_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
-        } else if (s.kind == 9) {
-            const int Dm = static_cast<int>(s.shape[0] / 3);
-            dit_qkv_bias_repack_kernel<<<blocks_for(static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1), 256>>>(
-                ctx->staging, static_cast<float*>(s.dst), Dm, s.aux0, s.aux1);
-        } else if (s.kind == 10) {
-            const int Dm = static_cast<int>(s.shape[0]);
-            const size_t out_n = static_cast<size_t>(Dm) * (Dm / s.aux0) * s.aux1;
-            dit_proj_weight_pad_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
-        } else if (s.kind == 7) {
-            float h[4] = {0.f, 0.f, 0.f, 0.f};
-            CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
-            for (float v : h)
-                if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
-        } else {
-            f32_to_bf16_kernel<<<blocks_for((s.numel + 3) / 4), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), s.numel);
+        switch (s.xform) {
+            case Xform::F32:
+                break;
+            case Xform::BF16:
+                f32_to_bf16_kernel<<<blocks_for((s.numel + 3) / 4), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), s.numel);
+                break;
+            case Xform::CONV_BF16: {
+                const int taps = static_cast<int>(s.shape[2] * s.shape[3]);
+                conv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
+                                                                       static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), taps);
+                break;
+            }
+            case Xform::TRANSPOSE_F32: {
+                const int r0 = static_cast<int>(s.shape[0]);
+                transpose_f32_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst), r0,
+                                                                  static_cast<int>(s.numel / r0));
+                break;
+            }
+            case Xform::EDM_QKV_W:
+                edm_qkv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
+                                                                          static_cast<int>(s.shape[1]), s.aux0, s.aux1);
+                break;
+            case Xform::EDM_QKV_B:
+                edm_qkv_bias_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst),
+                                                                        static_cast<int>(s.shape[0] / 3), s.aux0, s.aux1);
+                break;
+            case Xform::RESAMPLE_FILTER: {
+                float h[4] = {0.f, 0.f, 0.f, 0.f};
+                CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
+                for (float v : h)
+                    if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
+                break;
+            }
+            case Xform::DIT_QKV_W: {  // the destination has 3 * heads * aux1 rows
+                const int Dm = static_cast<int>(s.shape[1]);
+                const size_t out_n = static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1 * Dm;
+                dit_qkv_weight_repack_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
+                break;
+            }
+            case Xform::DIT_QKV_B: {
+                const int Dm = static_cast<int>(s.shape[0] / 3);
+                dit_qkv_bias_repack_kernel<<<blocks_for(static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1), 256>>>(
+                    ctx->staging, static_cast<float*>(s.dst), Dm, s.aux0, s.aux1);
+                break;
+            }
+            case Xform::DIT_PROJ_PAD: {
+                const int Dm = static_cast<int>(s.shape[0]);
+                const size_t out_n = static_cast<size_t>(Dm) * (Dm / s.aux0) * s.aux1;
+                dit_proj_weight_pad_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
+                break;
+            }
         }
         CUDA_OK(cudaGetLastError());
         CUDA_OK(cudaDeviceSynchronize());
@@ -527,9 +588,8 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
         if (!kv.second.set) return fail(ctx, "lfm_finalize: missing key '%s' (strict)", kv.first.c_str());
     if (ctx->finalized && max_batch <= ctx->max_rows) return 0;
     if (ctx->finalized) return fail(ctx, "lfm_finalize: already finalized for %d rows; create a new ctx for %d", ctx->max_rows, max_batch);
-    CUDA_OK(cudaSetDevice(ctx->device));
-    g_num_sms = ctx->num_sms;
-    if (ctx->arch == LFM_ARCH_UNET) {
+    if (bind(ctx)) return 1;
+    if (ctx->net != NetKind::DIT) {
         if (unet_finalize(ctx, max_batch)) return 1;
         if (alloc_solver_state(ctx, max_batch)) return 1;
         ctx->max_rows = max_batch;
@@ -578,22 +638,21 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
         CUDA_OK(cudaGetLastError());                  \
         ctx->launches++;                              \
     } while (0)
-#define LAUNCH_K(...)                                 \
+#define COUNT_LAUNCH(call)                            \
     do {                                              \
-        CUDA_OK(launch_k(__VA_ARGS__));               \
+        CUDA_OK(call);                                \
         ctx->launches++;                              \
     } while (0)
+#define LAUNCH_K(...) COUNT_LAUNCH(launch_k(__VA_ARGS__))
 
 static int check_ready(lfm_ctx* ctx, int rows, const char* who);
 
 #include "unet_host.inc"
 #include "vae_host.inc"
 
-static int ctx_unet_variant(const lfm_ctx* ctx) { return ctx->un != nullptr ? ctx->un->variant : 0; }
-
 static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int x_rows,
                           const long long* y, int rows) {
-    if (ctx->arch == LFM_ARCH_UNET) return launch_unet(ctx, s, t, t_numel, x, x_rows, y, rows);
+    if (ctx->net != NetKind::DIT) return launch_unet(ctx, s, t, t_numel, x, x_rows, y, rows);
     const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T, Dq = ctx->Dq;
     const int M = rows * T;
     // Conditioning c = t_emb(t) + y_emb(y) and the adaLN tables.  A 0-d t with y = None (every unconditional
@@ -611,8 +670,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     LAUNCH_OK();
     {   // all adaLN modulation vectors of the network in one GEMM: mod[crows, (6L+2) D]
         GemmEpi ep{ctx->b_mod, ctx->mod, ctx->Nmod, nullptr, 0, 1};
-        CUDA_OK(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
-        ctx->launches++;
+        COUNT_LAUNCH(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
     }
     const int ps = ctx->d.patch_size;
     if (ps == 2) {
@@ -635,49 +693,38 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     for (int l = 0; l < L; ++l) {
         BlockW& b = ctx->blk[l];
         const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
-        {
-            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, next_dir()));
-            ctx->launches++;
-        }
+        COUNT_LAUNCH(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, next_dir()));
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, 0, ep));
-            ctx->launches++;
+            COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, 0, ep));
         }
         {
             next_dir();  // attention reads each (sample, head) once: the sweep direction only keeps the GEMMs alternating
             // head_dim 64 keeps the kernel's own ch^-1/2; the padded DiT-XL heads pass the true head_dim^-1/2
             const float sc = 1.4426950408889634f / sqrtf(static_cast<float>(ctx->dh));
             if (!ctx->qkv_head_major)                          // 256 tokens, head_dim 64: TMA + wgmma
-                CUDA_OK(launch_attention_wgmma(s, ctx->tm_qkv_attn, ctx->attn, Dq, ctx->H, rows));
+                COUNT_LAUNCH(launch_attention_wgmma(s, ctx->tm_qkv_attn, ctx->attn, Dq, ctx->H, rows));
             else if (T == 16 || T == 64)                       // 4 x 4 / 8 x 8 token grids: the whole sequence in registers
-                CUDA_OK(launch_attention_mma(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, ctx->dh == 64 ? 0.f : sc));
+                COUNT_LAUNCH(launch_attention_mma(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, ctx->dh == 64 ? 0.f : sc));
             else                                               // 1024 tokens, head_dim 72: keys streamed in chunks of 64
-                CUDA_OK(launch_attention_flash(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, sc, false));
-            ctx->launches++;
+                COUNT_LAUNCH(launch_attention_flash(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, sc, false));
         }
         {
             GemmEpi ep{b.b_proj, ctx->x_tok, D, mb + 2 * D, Nmod, T};  // x += gate_msa * proj(...)   (models/DiT.py:129)
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
-            ctx->launches++;
+            COUNT_LAUNCH(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
         }
-        {
-            CUDA_OK(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, next_dir()));
-            ctx->launches++;
-        }
+        COUNT_LAUNCH(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, next_dir()));
         {
             GemmEpi ep{b.b_fc1, ctx->hmid, Hd, nullptr, 0, T};
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, 0, ep));
-            ctx->launches++;
+            COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, 0, ep));
         }
         {
             GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};  // x += gate_mlp * fc2(...)   (models/DiT.py:130)
             ep.reverse_m = next_dir();
-            CUDA_OK(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
-            ctx->launches++;
+            COUNT_LAUNCH(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
         }
     }
     {
@@ -704,7 +751,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
 static int eval_velocity(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int n_img,
                          const long long* y, float cfg_scale, int dup, float* v_out) {
     const size_t n = (size_t)n_img * ctx->chw;
-    if (cfg_scale > 1.0f && ctx->arch == LFM_ARCH_UNET && ctx_unet_variant(ctx) == 0)
+    if (cfg_scale > 1.0f && ctx->net == NetKind::ADM)
         return fail(ctx, "UNetModel has no forward_with_cfg (reference models/guided_diffusion/unet.py): cfg_scale must be <= 1");
     if (cfg_scale > 1.0f) {
         if (launch_network(ctx, s, t, t_numel, x, n_img, y, 2 * n_img)) return 1;
@@ -725,13 +772,19 @@ static int check_ready(lfm_ctx* ctx, int rows, const char* who) {
     return 0;
 }
 
+// check_ready for the entries that evaluate the velocity network (lfm_forward, lfm_sample_*), which a VAE context has not.
+static int check_velocity_ready(lfm_ctx* ctx, int rows, const char* who) {
+    if (check_ready(ctx, rows, who)) return 1;
+    if (ctx->net == NetKind::VAE) return fail(ctx, "%s: a VAE context (lfm_create_vae) has no velocity network", who);
+    return 0;
+}
+
 extern "C" int lfm_forward(lfm_ctx* ctx, const float* t, int t_numel, const float* x, const int64_t* y, int B,
                            float cfg_scale, float* v_out, void* stream) {
-    if (check_ready(ctx, B, "lfm_forward")) return 1;
+    if (check_velocity_ready(ctx, B, "lfm_forward")) return 1;
     if (t == nullptr || x == nullptr || v_out == nullptr) return fail(ctx, "lfm_forward: null tensor");
     if (t_numel != 1 && t_numel != B) return fail(ctx, "lfm_forward: t has %d elements, expected 1 or %d", t_numel, B);
-    CUDA_OK(cudaSetDevice(ctx->device));
-    g_num_sms = ctx->num_sms;
+    if (bind(ctx)) return 1;
     const bool cfg = cfg_scale > 1.0f;
     if (cfg && B % 2 != 0) return fail(ctx, "lfm_forward: forward_with_cfg needs an even batch (got %d)", B);
     // under CFG a vector t has 2n entries in the reference; both halves carry the same times (the x halves are identical)
@@ -838,15 +891,14 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     const int perturb = (t_as_vector & LFM_FIXED_PERTURB) ? 1 : 0;
     if (perturb && method == LFM_METHOD_HEUN) return fail(ctx, "lfm_sample_fixed: perturb applies to the torchdiffeq grids (euler, midpoint, rk4)");
     const int rows = cfg_scale > 1.0f ? 2 * B_img : B_img;
-    if (check_ready(ctx, rows, "lfm_sample_fixed")) return 1;
+    if (check_velocity_ready(ctx, rows, "lfm_sample_fixed")) return 1;
     if (method < LFM_METHOD_EULER || method > LFM_METHOD_RK4) return fail(ctx, "lfm_sample_fixed: unknown method %d", method);
     if (n_grid < 2 || n_grid > 8192) return fail(ctx, "lfm_sample_fixed: n_grid must be in [2, 8192] (got %d)", n_grid);
     if (x_inout == nullptr || t_grid_host == nullptr) return fail(ctx, "lfm_sample_fixed: null tensor");
     if (cfg_scale > 1.0f && y == nullptr) return fail(ctx, "lfm_sample_fixed: CFG needs labels");
     const int n_int = n_grid - 1, S = method == LFM_METHOD_EULER ? 1 : method == LFM_METHOD_RK4 ? 4 : 2;
     if (method >= LFM_METHOD_MIDPOINT && n_int * S > 8192) return fail(ctx, "lfm_sample_fixed: too many stages (%d)", n_int * S);
-    CUDA_OK(cudaSetDevice(ctx->device));
-    g_num_sms = ctx->num_sms;
+    if (bind(ctx)) return 1;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     const size_t n = (size_t)B_img * ctx->chw;
     const bool has_y = y != nullptr;
@@ -1073,13 +1125,12 @@ extern "C" int lfm_sample_dopri5(lfm_ctx* ctx, float* x_inout, double t0, double
 extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, double t0, double t1, double rtol, double atol,
                                    const int64_t* y, int B_img, float cfg_scale, lfm_ode_stats* stats, void* stream) {
     const int rows = cfg_scale > 1.0f ? 2 * B_img : B_img;
-    if (check_ready(ctx, rows, "lfm_sample_adaptive")) return 1;
+    if (check_velocity_ready(ctx, rows, "lfm_sample_adaptive")) return 1;
     if (method < LFM_ADAPTIVE_DOPRI5 || method > LFM_ADAPTIVE_HEUN) return fail(ctx, "lfm_sample_adaptive: unknown method %d", method);
     if (x_inout == nullptr) return fail(ctx, "lfm_sample_adaptive: null tensor");
     if (!(t0 > t1)) return fail(ctx, "lfm_sample_adaptive: expects t0 > t1 (reference integrates t: 1 -> 0)");
     if (cfg_scale > 1.0f && y == nullptr) return fail(ctx, "lfm_sample_adaptive: CFG needs labels");
-    CUDA_OK(cudaSetDevice(ctx->device));
-    g_num_sms = ctx->num_sms;
+    if (bind(ctx)) return 1;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     if (join_in(ctx, user)) return 1;
     Dopri d{ctx, ctx->stream, B_img, nullptr, cfg_scale, (size_t)B_img * ctx->chw};
@@ -1226,250 +1277,244 @@ extern "C" void lfm_destroy(lfm_ctx* ctx) {
 // ------------------------------------------------------------------------------------------------
 // kernel-level test entry points
 
+// Runs one kernel-level entry's launches, `op(ctx)`, on the current device, after its arguments are checked.  `ctx` stands in
+// for the network context: it receives the error message and counts the launches.
+template <typename Op>
+static int dbg_run(Op&& op) {
+    g_num_sms = query_num_sms();
+    if (g_num_sms <= 0) return fail(nullptr, "no CUDA device");
+    lfm_ctx dbg;
+    return op(&dbg);
+}
+
 extern "C" int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
                             int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n,
                             void* stream) {
-    lfm_ctx* ctx = nullptr;
-    if (K % 64 != 0 || N % 8 != 0) return fail(ctx, "lfm_dbg_gemm: K must be a multiple of 64 and N of 8");
-    if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(ctx, "lfm_dbg_gemm: unknown epilogue %d", epi);
+    if (K % 64 != 0 || N % 8 != 0) return fail(nullptr, "lfm_dbg_gemm: K must be a multiple of 64 and N of 8");
+    if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(nullptr, "lfm_dbg_gemm: unknown epilogue %d", epi);
     if (block_n != 0 && block_n != 128 && block_n != 256)
-        return fail(ctx, "lfm_dbg_gemm: block_n must be 0, 128 or 256 (got %d)", block_n);
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    CUtensorMap ta, tb;
-    if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
-        return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
-    GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
-    CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
-    return 0;
+        return fail(nullptr, "lfm_dbg_gemm: block_n must be 0, 128 or 256 (got %d)", block_n);
+    return dbg_run([&](lfm_ctx* ctx) {
+        CUtensorMap ta, tb;
+        if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
+            return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
+        GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
+        CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
+        return 0;
+    });
 }
 
 extern "C" int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s,
                                  void* stream) {
-    lfm_ctx* ctx = nullptr;
-    if (variant != 0 && variant != 1) return fail(ctx, "lfm_dbg_attention: variant must be 0 (wgmma) or 1 (mma.sync flash)");
-    if (dbg_s != nullptr) return fail(ctx, "lfm_dbg_attention: dbg_s is not supported (pass NULL)");
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (variant == 0) {
-        CUtensorMap tq;
-        if (!make_tmap_bf16(&tq, qkv_bf16, (uint64_t)B * 256, (uint64_t)3 * H * 64, kGemmBoxRows))
-            return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
-        CUDA_OK(launch_attention_wgmma(s, tq, static_cast<__nv_bfloat16*>(out_bf16), H * 64, H, B));
-    } else {
-        const float sc = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e), head_dim = 64
-        CUDA_OK(launch_attention_flash(s, static_cast<const __nv_bfloat16*>(qkv_bf16), static_cast<__nv_bfloat16*>(out_bf16), 256, 64,
-                                       H * 64, H, B * H, sc, true));
-    }
-    return 0;
+    if (variant != 0 && variant != 1) return fail(nullptr, "lfm_dbg_attention: variant must be 0 (wgmma) or 1 (mma.sync flash)");
+    if (dbg_s != nullptr) return fail(nullptr, "lfm_dbg_attention: dbg_s is not supported (pass NULL)");
+    return dbg_run([&](lfm_ctx* ctx) {
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (variant == 0) {
+            CUtensorMap tq;
+            if (!make_tmap_bf16(&tq, qkv_bf16, (uint64_t)B * 256, (uint64_t)3 * H * 64, kGemmBoxRows))
+                return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
+            CUDA_OK(launch_attention_wgmma(s, tq, static_cast<__nv_bfloat16*>(out_bf16), H * 64, H, B));
+        } else {
+            const float sc = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e), head_dim = 64
+            CUDA_OK(launch_attention_flash(s, static_cast<const __nv_bfloat16*>(qkv_bf16), static_cast<__nv_bfloat16*>(out_bf16), 256,
+                                           64, H * 64, H, B * H, sc, true));
+        }
+        return 0;
+    });
 }
 
 extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream) {
-    lfm_ctx* ctx = nullptr;
     if (!(ch == 64 || ch == 80 || ch == 128 || ch == 256) || head_dim < 0 || head_dim > ch)
-        return fail(ctx, "lfm_dbg_attention_mma: ch must be 64, 80, 128 or 256 and 0 <= head_dim <= ch (got ch %d, head_dim %d)", ch, head_dim);
+        return fail(nullptr, "lfm_dbg_attention_mma: ch must be 64, 80, 128 or 256 and 0 <= head_dim <= ch (got ch %d, head_dim %d)", ch,
+                    head_dim);
     const bool short_grid = T == 16 || T == 64;
     if (!short_grid && !(T > 0 && T % 64 == 0 && (ch == 64 || ch == 80)))
-        return fail(ctx, "lfm_dbg_attention_mma: T must be 16 or 64, or a multiple of 64 with ch 64 / 80 (got T %d, ch %d)", T, ch);
-    if (B < 1 || H < 1) return fail(ctx, "lfm_dbg_attention_mma: B and H must be >= 1 (got %d, %d)", B, H);
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
+        return fail(nullptr, "lfm_dbg_attention_mma: T must be 16 or 64, or a multiple of 64 with ch 64 / 80 (got T %d, ch %d)", T, ch);
+    if (B < 1 || H < 1) return fail(nullptr, "lfm_dbg_attention_mma: B and H must be >= 1 (got %d, %d)", B, H);
     // head_dim 0: the short-grid kernel's own ch^-1/2 (what the UNets run); the flash kernel always takes the scale from the host
     const float sc = head_dim > 0 ? 1.4426950408889634f / sqrtf(static_cast<float>(head_dim))
                                   : (short_grid ? 0.f : 1.4426950408889634f / sqrtf(static_cast<float>(ch)));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv_bf16);
-    __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out_bf16);
-    if (short_grid)
-        CUDA_OK(launch_attention_mma(s, q, o, T, ch, H * ch, H, B * H, sc));
-    else
-        CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
-    return 0;
+    return dbg_run([&](lfm_ctx* ctx) {
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv_bf16);
+        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out_bf16);
+        if (short_grid)
+            CUDA_OK(launch_attention_mma(s, q, o, T, ch, H * ch, H, B * H, sc));
+        else
+            CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
+        return 0;
+    });
 }
 
-// The entries below run one op of the UNet program through the program's own construction (push_*) and launch (run_*_op)
-// helpers.  `dbg` stands in for the network context: it receives the error message and counts the launches.
-// The device half of lfm_dbg_conv / lfm_dbg_conv_wide, on checked arguments.  ksplit -1 keeps push_conv's plan.
-static int dbg_conv_launch(const char* who, const void* x_bf16, const void* w_bf16, const float* bias, void* out,
-                           unsigned long long* gn_bins, int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit,
-                           void* stream) {
-    lfm_ctx* ctx = nullptr;
-    const int out_hw = (side / stride) * (side / stride);
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    lfm_ctx dbg;
-    ctx = &dbg;
-    UNetState u;
-    if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16), bias,
-                   Cout, out, epi))
-        return fail(ctx, "%s: tensor map encode failed", who);
-    UOp& o = u.prog[0];
-    if (ksplit >= 1) {
-        o.ksplit = ksplit;
-        o.split_pitch = ksplit > 1 ? (B * out_hw + kGemmBlockM - 1) / kGemmBlockM * kGemmBlockM : 0;
-    }
-    if (o.ksplit > 1 && (block_n == 256 || gn_bins != nullptr))
-        return fail(ctx, "%s: the network splits K %d ways here: pass ksplit 1 for block_n 256 or gn_bins", who, o.ksplit);
-    if (gn_bins != nullptr) {
-        o.bins_slot = 0;
-        u.BINS = gn_bins;
-        u.bins_rows = B;
-    }
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (o.ksplit > 1) CUDA_OK(cudaMallocAsync(&u.SPLIT, (size_t)o.ksplit * o.split_pitch * o.N * sizeof(float), s));
-    const int rc = run_gemm_op(ctx, &u, o, s, B, block_n);
-    if (u.SPLIT != nullptr) CUDA_OK(cudaFreeAsync(u.SPLIT, s));
-    return rc;
-}
+// The entries below run one op of the UNet program through the program's own construction (push_*) and launch (run_*_op) helpers.
 
 static bool conv_out_side_ok(int s) { return s == 4 || s == 8 || s == 16 || s == 32 || s == 64 || s == 128 || s == 256; }
 
-extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B,
-                            int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
-    lfm_ctx* ctx = nullptr;
-    if (B < 1) return fail(ctx, "lfm_dbg_conv: B must be >= 1 (got %d)", B);
-    if (stride != 1 && stride != 2) return fail(ctx, "lfm_dbg_conv: stride must be 1 or 2 (got %d)", stride);
-    if (side % stride != 0 || !conv_out_side_ok(side / stride))
-        return fail(ctx, "lfm_dbg_conv: side %d with stride %d: the output side must be 4, 8, 16, 32, 64, 128 or 256", side, stride);
-    if (Cin < 64 || Cin % 64 != 0) return fail(ctx, "lfm_dbg_conv: Cin must be a positive multiple of 64 (got %d)", Cin);
-    if (!(Cout == 4 || (Cout >= 8 && Cout % 8 == 0))) return fail(ctx, "lfm_dbg_conv: Cout must be 4 or a multiple of 8 (got %d)", Cout);
-    if (block_n != 0 && block_n != 128 && block_n != 256)
-        return fail(ctx, "lfm_dbg_conv: block_n must be 0, 128 or 256 (got %d)", block_n);
+// lfm_dbg_conv and lfm_dbg_conv_wide: the argument checks, then the launch.  `wide` selects the geometry and split-K rule of
+// lfm_dbg_conv_wide (output side 256 or 512, stride 1, never split along K) instead of lfm_dbg_conv's (output side 4..256,
+// stride 1 or 2, ksplit -1 = push_conv's plan, 1 = none, or 2..8).
+static int dbg_conv(const char* who, bool wide, const void* x_bf16, const void* w_bf16, const float* bias, void* out,
+                    unsigned long long* gn_bins, int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit,
+                    void* stream) {
+    if (wide) {
+        if (side != 256 && side != 512) return fail(nullptr, "%s: side must be 256 or 512 (got %d)", who, side);
+        if (stride != 1) return fail(nullptr, "%s: stride must be 1 (got %d)", who, stride);
+        if (B < 1 || (long long)B * side * side > INT32_MAX)
+            return fail(nullptr, "%s: B must be >= 1 and B * side^2 below 2^31 output pixels (got B %d)", who, B);
+    } else {
+        if (B < 1) return fail(nullptr, "%s: B must be >= 1 (got %d)", who, B);
+        if (stride != 1 && stride != 2) return fail(nullptr, "%s: stride must be 1 or 2 (got %d)", who, stride);
+        if (side % stride != 0 || !conv_out_side_ok(side / stride))
+            return fail(nullptr, "%s: side %d with stride %d: the output side must be 4, 8, 16, 32, 64, 128 or 256", who, side, stride);
+    }
+    if (Cin < 64 || Cin % 64 != 0) return fail(nullptr, "%s: Cin must be a positive multiple of 64 (got %d)", who, Cin);
+    if (!(Cout == 4 || (Cout >= 8 && Cout % 8 == 0))) return fail(nullptr, "%s: Cout must be 4 or a multiple of 8 (got %d)", who, Cout);
+    if (block_n != 0 && block_n != 128 && block_n != 256) return fail(nullptr, "%s: block_n must be 0, 128 or 256 (got %d)", who, block_n);
     if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16 && epi != EPI_GATE_RESID_F32)
-        return fail(ctx, "lfm_dbg_conv: epi must be 3 (fp32 out), 0 (bf16 out) or 2 (out += conv) (got %d)", epi);
-    if (ksplit != -1 && (ksplit < 1 || ksplit > 8))
-        return fail(ctx, "lfm_dbg_conv: ksplit must be -1 (the network's plan), 1 (none) or 2..8 (got %d)", ksplit);
-    if (ksplit > 1 && (epi == EPI_BIAS_BF16 || block_n == 256))
-        return fail(ctx, "lfm_dbg_conv: ksplit %d: split-K writes fp32 (epi 3 or 2) with 128-wide tiles (block_n 0 or 128)", ksplit);
+        return fail(nullptr, "%s: epi must be 3 (fp32 out), 0 (bf16 out) or 2 (out += conv) (got %d)", who, epi);
+    if (wide) {
+        if (ksplit != 1) return fail(nullptr, "%s: ksplit must be 1: wide rows are never split along K (got %d)", who, ksplit);
+    } else {
+        if (ksplit != -1 && (ksplit < 1 || ksplit > 8))
+            return fail(nullptr, "%s: ksplit must be -1 (the network's plan), 1 (none) or 2..8 (got %d)", who, ksplit);
+        if (ksplit > 1 && (epi == EPI_BIAS_BF16 || block_n == 256))
+            return fail(nullptr, "%s: ksplit %d: split-K writes fp32 (epi 3 or 2) with 128-wide tiles (block_n 0 or 128)", who, ksplit);
+    }
     const int out_hw = (side / stride) * (side / stride), cpg = Cout / 32;
     if (gn_bins != nullptr && (epi == EPI_GATE_RESID_F32 || ksplit > 1 || Cout % 32 != 0 ||
                                !(cpg == 4 || cpg == 8 || cpg == 16 || cpg == 32 || cpg == 64) || out_hw % 32 != 0))
-        return fail(ctx, "lfm_dbg_conv: gn_bins needs epi 3 or 0, no split-K, Cout / 32 in {4, 8, 16, 32, 64} and a multiple of 32 "
-                         "output pixels (got epi %d, ksplit %d, Cout %d, %d pixels)", epi, ksplit, Cout, out_hw);
+        return fail(nullptr, "%s: gn_bins needs epi 3 or 0, no split-K, Cout / 32 in {4, 8, 16, 32, 64} and a multiple of 32 "
+                             "output pixels (got epi %d, ksplit %d, Cout %d, %d pixels)", who, epi, ksplit, Cout, out_hw);
     if (x_bf16 == nullptr || w_bf16 == nullptr || bias == nullptr || out == nullptr)
-        return fail(ctx, "lfm_dbg_conv: x, w, bias and out must not be NULL");
-    return dbg_conv_launch("lfm_dbg_conv", x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream);
+        return fail(nullptr, "%s: x, w, bias and out must not be NULL", who);
+    return dbg_run([&](lfm_ctx* ctx) {
+        UNetState u;
+        if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16),
+                       bias, Cout, out, epi))
+            return fail(ctx, "%s: tensor map encode failed", who);
+        UOp& o = u.prog[0];
+        if (ksplit >= 1) {
+            o.ksplit = ksplit;
+            o.split_pitch = ksplit > 1 ? (B * out_hw + kGemmBlockM - 1) / kGemmBlockM * kGemmBlockM : 0;
+        }
+        if (o.ksplit > 1 && (block_n == 256 || gn_bins != nullptr))
+            return fail(ctx, "%s: the network splits K %d ways here: pass ksplit 1 for block_n 256 or gn_bins", who, o.ksplit);
+        if (gn_bins != nullptr) {
+            o.bins_slot = 0;
+            u.BINS = gn_bins;
+            u.bins_rows = B;
+        }
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (o.ksplit > 1) CUDA_OK(cudaMallocAsync(&u.SPLIT, (size_t)o.ksplit * o.split_pitch * o.N * sizeof(float), s));
+        const int rc = run_gemm_op(ctx, &u, o, s, B, block_n);
+        if (u.SPLIT != nullptr) CUDA_OK(cudaFreeAsync(u.SPLIT, s));
+        return rc;
+    });
+}
+
+extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B,
+                            int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
+    return dbg_conv("lfm_dbg_conv", false, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream);
 }
 
 // Stride-1 3x3 convolutions whose output rows are wider than one 128-pixel tile (the row-segment tiles of the VAE decoder's
 // last stages): the same push_conv / run_gemm_op path, never split along K.
 extern "C" int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins,
                                  int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
-    lfm_ctx* ctx = nullptr;
-    if (side != 256 && side != 512) return fail(ctx, "lfm_dbg_conv_wide: side must be 256 or 512 (got %d)", side);
-    if (stride != 1) return fail(ctx, "lfm_dbg_conv_wide: stride must be 1 (got %d)", stride);
-    if (B < 1 || (long long)B * side * side > INT32_MAX)
-        return fail(ctx, "lfm_dbg_conv_wide: B must be >= 1 and B * side^2 below 2^31 output pixels (got B %d)", B);
-    if (Cin < 64 || Cin % 64 != 0) return fail(ctx, "lfm_dbg_conv_wide: Cin must be a positive multiple of 64 (got %d)", Cin);
-    if (!(Cout == 4 || (Cout >= 8 && Cout % 8 == 0))) return fail(ctx, "lfm_dbg_conv_wide: Cout must be 4 or a multiple of 8 (got %d)", Cout);
-    if (block_n != 0 && block_n != 128 && block_n != 256)
-        return fail(ctx, "lfm_dbg_conv_wide: block_n must be 0, 128 or 256 (got %d)", block_n);
-    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16 && epi != EPI_GATE_RESID_F32)
-        return fail(ctx, "lfm_dbg_conv_wide: epi must be 3 (fp32 out), 0 (bf16 out) or 2 (out += conv) (got %d)", epi);
-    if (ksplit != 1) return fail(ctx, "lfm_dbg_conv_wide: ksplit must be 1: wide rows are never split along K (got %d)", ksplit);
-    const int cpg = Cout / 32;
-    if (gn_bins != nullptr && (epi == EPI_GATE_RESID_F32 || Cout % 32 != 0 || !(cpg == 4 || cpg == 8 || cpg == 16 || cpg == 32 || cpg == 64)))
-        return fail(ctx, "lfm_dbg_conv_wide: gn_bins needs epi 3 or 0 and Cout / 32 in {4, 8, 16, 32, 64} (got epi %d, Cout %d)", epi, Cout);
-    if (x_bf16 == nullptr || w_bf16 == nullptr || bias == nullptr || out == nullptr)
-        return fail(ctx, "lfm_dbg_conv_wide: x, w, bias and out must not be NULL");
-    return dbg_conv_launch("lfm_dbg_conv_wide", x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, 1, block_n, epi, 1, stream);
+    return dbg_conv("lfm_dbg_conv_wide", true, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit,
+                    stream);
 }
 
 extern "C" int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w_bf16, int w_rows, int w_ld, int K, int N,
                                     void* out, const float* bias, int B, int out_hw, int epi, int batch_m, int a_mod, int b_batch_rows,
                                     void* stream) {
-    lfm_ctx* ctx = nullptr;
     if (K < 64 || K % 64 != 0 || N < 256 || N % 256 != 0)
-        return fail(ctx, "lfm_dbg_gemm_batched: K must be a multiple of 64 and N of 256 (got K %d, N %d)", K, N);
+        return fail(nullptr, "lfm_dbg_gemm_batched: K must be a multiple of 64 and N of 256 (got K %d, N %d)", K, N);
     if (a_rows < 1 || w_rows < 1 || a_ld < K || w_ld < K || a_ld % 8 != 0 || w_ld % 8 != 0)
-        return fail(ctx, "lfm_dbg_gemm_batched: a_ld / w_ld must be >= K and multiples of 8, a_rows / w_rows >= 1 "
-                         "(got a %d x ld %d, w %d x ld %d)", a_rows, a_ld, w_rows, w_ld);
+        return fail(nullptr, "lfm_dbg_gemm_batched: a_ld / w_ld must be >= K and multiples of 8, a_rows / w_rows >= 1 "
+                             "(got a %d x ld %d, w %d x ld %d)", a_rows, a_ld, w_rows, w_ld);
     if (batch_m < 128 || batch_m % 128 != 0 || a_mod < 0 || a_mod % 128 != 0 || b_batch_rows < N)
-        return fail(ctx, "lfm_dbg_gemm_batched: batch_m must be a positive multiple of 128, a_mod 0 or a multiple of 128, "
-                         "b_batch_rows >= N (got batch_m %d, a_mod %d, b_batch_rows %d)", batch_m, a_mod, b_batch_rows);
+        return fail(nullptr, "lfm_dbg_gemm_batched: batch_m must be a positive multiple of 128, a_mod 0 or a multiple of 128, "
+                             "b_batch_rows >= N (got batch_m %d, a_mod %d, b_batch_rows %d)", batch_m, a_mod, b_batch_rows);
     if (B < 1 || out_hw < 1 || ((long long)B * out_hw) % batch_m != 0)
-        return fail(ctx, "lfm_dbg_gemm_batched: B * out_hw must be a positive multiple of batch_m (got %d x %d)", B, out_hw);
-    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16) return fail(ctx, "lfm_dbg_gemm_batched: epi must be 3 (fp32) or 0 (bf16) (got %d)", epi);
-    if (a_bf16 == nullptr || w_bf16 == nullptr || out == nullptr) return fail(ctx, "lfm_dbg_gemm_batched: a, w and out must not be NULL");
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    lfm_ctx dbg;
-    ctx = &dbg;
-    UNetState u;
-    if (!push_batched(&u, a_bf16, a_rows, a_ld, K, w_bf16, w_rows, w_ld, N, out, out_hw, epi, bias, batch_m, a_mod, b_batch_rows))
-        return fail(ctx, "lfm_dbg_gemm_batched: tensor map encode failed");
-    return run_gemm_op(ctx, &u, u.prog[0], static_cast<cudaStream_t>(stream), B, 0);
+        return fail(nullptr, "lfm_dbg_gemm_batched: B * out_hw must be a positive multiple of batch_m (got %d x %d)", B, out_hw);
+    if (epi != EPI_BIAS_F32 && epi != EPI_BIAS_BF16)
+        return fail(nullptr, "lfm_dbg_gemm_batched: epi must be 3 (fp32) or 0 (bf16) (got %d)", epi);
+    if (a_bf16 == nullptr || w_bf16 == nullptr || out == nullptr)
+        return fail(nullptr, "lfm_dbg_gemm_batched: a, w and out must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        UNetState u;
+        if (!push_batched(&u, a_bf16, a_rows, a_ld, K, w_bf16, w_rows, w_ld, N, out, out_hw, epi, bias, batch_m, a_mod, b_batch_rows))
+            return fail(ctx, "lfm_dbg_gemm_batched: tensor map encode failed");
+        return run_gemm_op(ctx, &u, u.prog[0], static_cast<cudaStream_t>(stream), B, 0);
+    });
 }
 
 extern "C" int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb, const void* src_bf16, const unsigned long long* bins,
                                  int max_chunks, const float* gamma, const float* beta, const float* film, int film_stride, int act,
                                  float eps, void* out_bf16, float* copy_out, void* raw_out, int B, int HW, void* stream) {
-    lfm_ctx* ctx = nullptr;
     const int C = Ca + Cb;
     if (Ca < 4 || Ca % 4 != 0 || Cb < 0 || Cb % 4 != 0 || (b == nullptr) != (Cb == 0))
-        return fail(ctx, "lfm_dbg_groupnorm: Ca must be a positive multiple of 4, Cb 0 (b NULL) or a multiple of 4 (got %d, %d)", Ca, Cb);
-    if (C % 128 != 0 || C > 128 * kGnMaxJ) return fail(ctx, "lfm_dbg_groupnorm: Ca + Cb must be a multiple of 128 up to %d (got %d)", 128 * kGnMaxJ, C);
-    if (B < 1 || B > 65535 || HW < 1) return fail(ctx, "lfm_dbg_groupnorm: B must be in [1, 65535] and HW >= 1 (got %d, %d)", B, HW);
+        return fail(nullptr, "lfm_dbg_groupnorm: Ca must be a positive multiple of 4, Cb 0 (b NULL) or a multiple of 4 (got %d, %d)", Ca, Cb);
+    if (C % 128 != 0 || C > 128 * kGnMaxJ)
+        return fail(nullptr, "lfm_dbg_groupnorm: Ca + Cb must be a multiple of 128 up to %d (got %d)", 128 * kGnMaxJ, C);
+    if (B < 1 || B > 65535 || HW < 1) return fail(nullptr, "lfm_dbg_groupnorm: B must be in [1, 65535] and HW >= 1 (got %d, %d)", B, HW);
     if (bins == nullptr && (max_chunks < 1 || max_chunks > 256))
-        return fail(ctx, "lfm_dbg_groupnorm: max_chunks must be in [1, 256] (got %d)", max_chunks);
-    if (act != 0 && act != 1) return fail(ctx, "lfm_dbg_groupnorm: act must be 0 or 1 (SiLU) (got %d)", act);
-    if (film_stride < 0 || !(eps > 0.f)) return fail(ctx, "lfm_dbg_groupnorm: film_stride must be >= 0 and eps > 0");
+        return fail(nullptr, "lfm_dbg_groupnorm: max_chunks must be in [1, 256] (got %d)", max_chunks);
+    if (act != 0 && act != 1) return fail(nullptr, "lfm_dbg_groupnorm: act must be 0 or 1 (SiLU) (got %d)", act);
+    if (film_stride < 0 || !(eps > 0.f)) return fail(nullptr, "lfm_dbg_groupnorm: film_stride must be >= 0 and eps > 0");
     if (a == nullptr || gamma == nullptr || beta == nullptr || out_bf16 == nullptr)
-        return fail(ctx, "lfm_dbg_groupnorm: a, gamma, beta and out must not be NULL");
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    lfm_ctx dbg;
-    ctx = &dbg;
-    UNetState u;
-    u.gn_eps = eps;
-    u.max_chunks = max_chunks;
-    push_gn(&u, Src2{a, b, Ca, Cb}, HW, C, gamma, beta, film != nullptr ? 0 : -1, act, static_cast<__nv_bfloat16*>(out_bf16), copy_out,
-            static_cast<__nv_bfloat16*>(raw_out));
-    u.film = const_cast<float*>(film);
-    UOp& st = u.prog[0];
-    UOp& ap = u.prog[1];
-    ap.gn_src_bf16 = static_cast<const __nv_bfloat16*>(src_bf16);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (bins != nullptr) {  // statistics from a producing convolution's epilogue: [B][kGnBinReplicas][32 groups][sum, sum of squares]
-        st.skip = true;
-        ap.bins_slot = 0;
-        u.BINS = const_cast<unsigned long long*>(bins);
-        u.bins_rows = B;
-    } else {
-        CUDA_OK(cudaMallocAsync(&u.partial, (size_t)B * max_chunks * 64 * sizeof(double), s));
-    }
-    int rc = 0;
-    for (const UOp& o : u.prog)
-        if (rc == 0 && !o.skip) rc = run_gn_op(ctx, &u, o, s, B, film_stride);
-    if (u.partial != nullptr) CUDA_OK(cudaFreeAsync(u.partial, s));
-    return rc;
+        return fail(nullptr, "lfm_dbg_groupnorm: a, gamma, beta and out must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        UNetState u;
+        u.gn_eps = eps;
+        u.max_chunks = max_chunks;
+        push_gn(&u, Src2{a, b, Ca, Cb}, HW, C, gamma, beta, film != nullptr ? 0 : -1, act, static_cast<__nv_bfloat16*>(out_bf16),
+                copy_out, static_cast<__nv_bfloat16*>(raw_out));
+        u.film = const_cast<float*>(film);
+        UOp& st = u.prog[0];
+        UOp& ap = u.prog[1];
+        ap.gn_src_bf16 = static_cast<const __nv_bfloat16*>(src_bf16);
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (bins != nullptr) {  // statistics from a producing convolution's epilogue: [B][kGnBinReplicas][32 groups][sum, sum of squares]
+            st.skip = true;
+            ap.bins_slot = 0;
+            u.BINS = const_cast<unsigned long long*>(bins);
+            u.bins_rows = B;
+        } else {
+            CUDA_OK(cudaMallocAsync(&u.partial, (size_t)B * max_chunks * 64 * sizeof(double), s));
+        }
+        int rc = 0;
+        for (const UOp& o : u.prog)
+            if (rc == 0 && !o.skip) rc = run_gn_op(ctx, &u, o, s, B, film_stride);
+        if (u.partial != nullptr) CUDA_OK(cudaFreeAsync(u.partial, s));
+        return rc;
+    });
 }
 
 extern "C" int lfm_dbg_unet_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int C, int heads, void* stream) {
-    lfm_ctx* ctx = nullptr;
     if (B < 1 || heads < 1 || C % heads != 0)
-        return fail(ctx, "lfm_dbg_unet_attention: B and heads must be >= 1 and C a multiple of heads (got B %d, C %d, heads %d)", B, C, heads);
+        return fail(nullptr, "lfm_dbg_unet_attention: B and heads must be >= 1 and C a multiple of heads (got B %d, C %d, heads %d)", B, C,
+                    heads);
     if (!unet_attn_supported(T, C / heads))
-        return fail(ctx, "lfm_dbg_unet_attention: %d tokens with a head width of %d channels is not supported", T, C / heads);
-    if (qkv_bf16 == nullptr || out_bf16 == nullptr) return fail(ctx, "lfm_dbg_unet_attention: qkv and out must not be NULL");
-    g_num_sms = query_num_sms();
-    if (g_num_sms <= 0) return fail(ctx, "no CUDA device");
-    lfm_ctx dbg;
-    ctx = &dbg;
-    UOp o;
-    o.kind = U_ATTN;
-    o.qkv = static_cast<const __nv_bfloat16*>(qkv_bf16);
-    o.att = static_cast<__nv_bfloat16*>(out_bf16);
-    o.HW = T;
-    o.C = C;
-    o.heads = heads;
-    return run_attn_op(ctx, o, static_cast<cudaStream_t>(stream), B);
+        return fail(nullptr, "lfm_dbg_unet_attention: %d tokens with a head width of %d channels is not supported", T, C / heads);
+    if (qkv_bf16 == nullptr || out_bf16 == nullptr) return fail(nullptr, "lfm_dbg_unet_attention: qkv and out must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        UOp o;
+        o.kind = U_ATTN;
+        o.qkv = static_cast<const __nv_bfloat16*>(qkv_bf16);
+        o.att = static_cast<__nv_bfloat16*>(out_bf16);
+        o.HW = T;
+        o.C = C;
+        o.heads = heads;
+        return run_attn_op(ctx, o, static_cast<cudaStream_t>(stream), B);
+    });
 }
 
 extern "C" int lfm_dbg_tokens(lfm_ctx* ctx, float* out, int B) {
     if (check_ready(ctx, B, "lfm_dbg_tokens")) return 1;
-    if (ctx->arch != LFM_ARCH_DIT) return fail(ctx, "lfm_dbg_tokens: DiT only");
+    if (ctx->net != NetKind::DIT) return fail(ctx, "lfm_dbg_tokens: DiT only");
     CUDA_OK(cudaMemcpy(out, ctx->x_tok, (size_t)B * ctx->T * ctx->D * sizeof(float), cudaMemcpyDefault));
     return 0;
 }

@@ -823,15 +823,6 @@ __global__ void conv_weight_repack_kernel(const float* __restrict__ w, __nv_bflo
     const int o = static_cast<int>(i / (static_cast<size_t>(Cin) * taps));
     out[i] = __float2bfloat16(w[(static_cast<size_t>(o) * Cin + c) * taps + tap]);
 }
-// out.2 weight repack: [4, C, 3, 3] fp32 -> [4][9][C] fp32
-__global__ void conv_out_weight_repack_kernel(const float* __restrict__ w, float* __restrict__ out, int C) {
-    const int n = 4 * 9 * C;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int c = i % C, tap = (i / C) % 9, o = i / (9 * C);
-    out[i] = w[(static_cast<size_t>(o) * C + c) * 9 + tap];
-}
-
 // sinusoidal timestep features of arbitrary even width (nn.py:103-121; cos first, raw t)
 __global__ void timestep_features_dim_kernel(const float* __restrict__ t, int t_numel, float* __restrict__ tf, int B, int dim) {
     pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line

@@ -712,6 +712,32 @@ def test_vae_mid_attention_and_stage_features(dev):
     assert torch.equal(vae.decode(z.to(dev)).sample.cpu(), base)
 
 
+def test_vae_context_refuses_the_velocity_entries(dev):
+    """A VAE context has no velocity network: lfm_forward, lfm_sample_fixed and lfm_sample_adaptive refuse it and say so, before
+    they launch anything, and the context decodes as before afterwards."""
+    vae, _ = make_vae(dev)
+    z = torch.randn(1, 4, 16, 16, generator=torch.Generator().manual_seed(6)).to(dev)
+    base = vae.decode(z).sample
+    ctx = vae.native(1, dev)
+    lib = _lib.load()
+    launches = lib.lfm_launch_count(ctx)
+    x, v = z.clone(), torch.empty_like(z)
+    t = torch.full((1,), 0.5, device=dev)
+    grid = torch.tensor([1.0, 0.5, 0.0])
+    calls = {
+        "lfm_forward": lambda: lib.lfm_forward(ctx, t.data_ptr(), 1, x.data_ptr(), None, 1, 1.0, v.data_ptr(), None),
+        "lfm_sample_fixed": lambda: lib.lfm_sample_fixed(ctx, 0, x.data_ptr(), grid.data_ptr(), 3, 0, 0, None, 1, 1.0, None, None),
+        "lfm_sample_adaptive": lambda: lib.lfm_sample_adaptive(ctx, 0, x.data_ptr(), 1.0, 0.0, 1e-5, 1e-5, None, 1, 1.0, None, None),
+    }
+    for who, call in calls.items():
+        assert call() != 0, who
+        msg = _lib.last_error(ctx)
+        assert who in msg and "VAE context" in msg and "no velocity network" in msg, msg
+    torch.cuda.synchronize()
+    assert lib.lfm_launch_count(ctx) == launches and torch.equal(x, z)
+    assert torch.equal(vae.decode(z).sample, base)
+
+
 # ------------------------------------------------------------------------------------------------ edges / CLI
 
 
