@@ -52,7 +52,7 @@ typedef struct lfm_model_desc {
  * use_scale_shift_norm = True, resblock_updown = False, conv_resample = True, legacy attention order, dims = 2. */
 typedef struct lfm_unet_desc {
     int32_t image_size;                /* latent side (config.image_size // 8), e.g. 64 */
-    int32_t in_channels;               /* 4 */
+    int32_t in_channels;               /* 4, or 5..16: concat-conditioned (see lfm_set_condition) */
     int32_t model_channels;            /* nf, multiple of 128 */
     int32_t out_channels;              /* 4 */
     int32_t num_res_blocks;
@@ -109,6 +109,17 @@ int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out);
  * lfm_set_param / lfm_finalize / lfm_forward / lfm_sample_* entry points then operate on the UNet
  * (model(t, x, y) = UNetModel.forward, unet.py:613-655; it has no forward_with_cfg: cfg_scale must be <= 1). */
 int lfm_create_unet(const lfm_unet_desc* desc, int device, lfm_ctx** out);
+
+/* Concat-conditioned UNetModel (in_channels in [5, 16], out_channels 4): the downstream tasks' WrapperCondFlow,
+ * model(t, cat([x, cond], 1)) (downstream_tasks/test_flow_latent_inpainting.py, test_flow_latent_semantic_syn.py).
+ * Copies cond [B_img, channels, H, W] fp32 NCHW (device), channels = in_channels - out_channels, into the context, ordered on
+ * `stream`.  The samplers then evolve the [B_img, 4, H, W] state and evaluate the network on [state | cond]; they refuse to run
+ * unless the stored condition holds exactly B_img images.  Their adaptive error norm covers the state only (torchdiffeq
+ * integrates x; the concatenation happens inside the field).  The condition lives at a fixed address, so the cached step graphs
+ * read each new condition.  lfm_forward on such a context takes x as the whole input [B, in_channels, H, W] and writes
+ * v_out [B, 4, H, W]; it does not read the stored condition.  Refused on an unconditioned or unfinalized context, on a wrong
+ * `channels` and on B_img above the finalized rows. */
+int lfm_set_condition(lfm_ctx* ctx, const float* cond, int B_img, int channels, void* stream);
 
 /* models/__init__.py:10-11 create_network(config) -> get_edm_network(config) -> DhariwalUNet (EDM.py:906-921).
  * The same lfm_set_param / lfm_finalize / lfm_forward / lfm_sample_* entry points then operate on it:
@@ -217,6 +228,12 @@ int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void
  * lfm_dbg_conv.  Arguments are checked before the device is touched. */
 int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
                       int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
+/* The UNet programs' conv_in (3x3, pad 1, fp32) as the network runs it: input channels [a | b] of two NCHW fp32 sources, a with a_ch
+ * channels and image i at a + i * a_stride, b likewise (NULL when b_ch = 0); a_ch + b_ch in [3, 16].  w fp32 [Cout, a_ch + b_ch, 3, 3],
+ * bias fp32 [Cout], out fp32 NHWC [B, side, side, Cout].  side in [1, 256] (with (a_ch + b_ch) * 3 * (side + 4) floats in 48 KB).
+ * Arguments are checked before the device is touched. */
+int lfm_dbg_conv_in(const float* a, int a_ch, long long a_stride, const float* b, int b_ch, long long b_stride, const float* w,
+                    const float* bias, float* out, int B, int side, int Cout, void* stream);
 /* The batched GEMM of the VAE mid-block attention: M = B * out_hw rows in groups of batch_m; group g computes
  * out[g rows] = A[rows] W[g * b_batch_rows .. + N]^T (+ bias), A row = row % a_mod when a_mod > 0 (A shared by all groups).
  * a: bf16 [a_rows, K] with row pitch a_ld, w: bf16 [w_rows, K] with row pitch w_ld (column windows of wider matrices);

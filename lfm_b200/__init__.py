@@ -9,8 +9,9 @@ from .network import DiT, DiT_models, create_network, get_flow_model  # noqa: F4
 from .unet import UNetModel  # noqa: F401
 from .edm import DhariwalUNet, get_edm_network  # noqa: F401
 from .vae import AutoencoderKL, synthetic_vae_state_dict  # noqa: F401
+from .downstream import SpatialRescaler, WrapperCondFlow  # noqa: F401
 from .solvers import (ADAPTIVE_SOLVER, FIXER_SOLVER, euler_time_grid, karras_sample, sample_from_model,  # noqa: F401
                       sample_from_model_with_fixed_step_solve, sample_from_model_with_fixed_step_solver)
 
 __all__ = ["DiT", "UNetModel", "DhariwalUNet", "AutoencoderKL", "get_edm_network", "DiT_models", "create_network", "get_flow_model", "karras_sample", "sample_from_model",
-           "sample_from_model_with_fixed_step_solver", "euler_time_grid"]
+           "sample_from_model_with_fixed_step_solver", "euler_time_grid", "WrapperCondFlow", "SpatialRescaler"]

@@ -48,6 +48,7 @@ SYMBOLS = {
     "lfm_decode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "lfm_set_param": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.POINTER(C.c_int64), C.c_int]),
     "lfm_finalize": (C.c_int, [_P, C.c_int]),
+    "lfm_set_condition": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     "lfm_forward": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_float, _P, _P]),
     "lfm_sample_fixed": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_float,
                                    C.POINTER(OdeStats), _P]),
@@ -63,6 +64,7 @@ SYMBOLS = {
     "lfm_dbg_attention_mma": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv_wide": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_conv_in": (C.c_int, [_P, C.c_int, C.c_longlong, _P, C.c_int, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_gemm_batched": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int,
                                        C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_groupnorm": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P,

@@ -240,7 +240,8 @@ struct lfm_ctx {
     UNetState* un = nullptr;
     int device = 0;
     int num_sms = 0;
-    int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, Nmod = 0, HW = 0, chw = 0;
+    int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, Nmod = 0, HW = 0;
+    int in_chw = 0, out_chw = 0;  // floats of one image of the network input / of the solver state and the velocity
     int dh = 64, dhp = 64, Dq = 0;  // head_dim, its stored (zero-padded) width and the width H * dhp of the attention tensors
     bool qkv_head_major = false;    // qkv rows re-ordered head-major (everything but T = 256 with head_dim 64, see lfm_create)
     int max_rows = 0;
@@ -466,7 +467,7 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->C = desc->in_channels;
     ctx->Hd = desc->mlp_hidden;
     ctx->HW = desc->img_resolution;
-    ctx->chw = ctx->C * ctx->HW * ctx->HW;
+    ctx->in_chw = ctx->out_chw = ctx->C * ctx->HW * ctx->HW;
     ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
     // 256 tokens with head_dim 64 (every released preset) keep the checkpoint's timm qkv order, which the flash kernel reads directly.
     // Everything else - 16 / 64 / 1024 tokens, head_dim 72 (DiT-XL, stored padded to 80) - stores the qkv rows head-major.
@@ -559,7 +560,7 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
 
 static int alloc_solver_state(lfm_ctx* ctx, int R) {
     // solver state (sized for R latent rows)
-    const size_t nst = (size_t)R * ctx->chw;
+    const size_t nst = (size_t)R * ctx->out_chw;
     if (dev_alloc(ctx, &ctx->x_state, nst)) return 1;
     if (dev_alloc(ctx, &ctx->x_pred, nst)) return 1;
     if (dev_alloc(ctx, &ctx->y_stage, nst)) return 1;
@@ -608,7 +609,7 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (dev_alloc(ctx, &ctx->c_silu, (size_t)Rpad * D)) return 1;
     if (dev_alloc(ctx, &ctx->tfreq, (size_t)R * 256)) return 1;
     if (dev_alloc(ctx, &ctx->h1, (size_t)R * D)) return 1;
-    if (dev_alloc(ctx, &ctx->v_net, (size_t)R * ctx->chw)) return 1;
+    if (dev_alloc(ctx, &ctx->v_net, (size_t)R * ctx->out_chw)) return 1;
     if (alloc_solver_state(ctx, R)) return 1;
 
     bool ok = true;
@@ -650,9 +651,10 @@ static int check_ready(lfm_ctx* ctx, int rows, const char* who);
 #include "unet_host.inc"
 #include "vae_host.inc"
 
+// x_whole: see run_unet_program (conditioned UNets only)
 static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int x_rows,
-                          const long long* y, int rows) {
-    if (ctx->net != NetKind::DIT) return launch_unet(ctx, s, t, t_numel, x, x_rows, y, rows);
+                          const long long* y, int rows, bool x_whole) {
+    if (ctx->net != NetKind::DIT) return launch_unet(ctx, s, t, t_numel, x, x_rows, y, rows, x_whole);
     const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T, Dq = ctx->Dq;
     const int M = rows * T;
     // Conditioning c = t_emb(t) + y_emb(y) and the adaLN tables.  A 0-d t with y = None (every unconditional
@@ -748,17 +750,18 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
 // Evaluate the (CFG-combined) velocity of n_img latents in `x` into `v_out` [n_img, C, H, W].
 //   cfg_scale > 1: network batch = 2 n_img rows (labels y[0:n] conditional, y[n:2n] null), v = u + s (c - u);
 //   dup != 0 writes v into both halves of v_out [2 n_img, C, H, W] (forward_with_cfg returns cat[v, v]).
+//   x_whole: x is the whole input of a conditioned network (see run_unet_program).
 static int eval_velocity(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int n_img,
-                         const long long* y, float cfg_scale, int dup, float* v_out) {
-    const size_t n = (size_t)n_img * ctx->chw;
+                         const long long* y, float cfg_scale, int dup, float* v_out, bool x_whole = false) {
+    const size_t n = (size_t)n_img * ctx->out_chw;
     if (cfg_scale > 1.0f && ctx->net == NetKind::ADM)
         return fail(ctx, "UNetModel has no forward_with_cfg (reference models/guided_diffusion/unet.py): cfg_scale must be <= 1");
     if (cfg_scale > 1.0f) {
-        if (launch_network(ctx, s, t, t_numel, x, n_img, y, 2 * n_img)) return 1;
+        if (launch_network(ctx, s, t, t_numel, x, n_img, y, 2 * n_img, x_whole)) return 1;
         cfg_combine_kernel<<<blocks_for(n), 256, 0, s>>>(ctx->v_net, v_out, n, cfg_scale, dup);
         LAUNCH_OK();
     } else {
-        if (launch_network(ctx, s, t, t_numel, x, n_img, y, n_img)) return 1;
+        if (launch_network(ctx, s, t, t_numel, x, n_img, y, n_img, x_whole)) return 1;
         CUDA_OK(cudaMemcpyAsync(v_out, ctx->v_net, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
     return 0;
@@ -779,6 +782,15 @@ static int check_velocity_ready(lfm_ctx* ctx, int rows, const char* who) {
     return 0;
 }
 
+// A concat-conditioned context (in_channels > out_channels) evaluates its network on [state | stored condition]: the samplers run
+// only with a condition for exactly their B_img images.
+static int check_condition(lfm_ctx* ctx, int B_img, const char* who) {
+    const UNetState* u = ctx->un;
+    if (u == nullptr || u->cond_ch == 0 || u->cond_rows == B_img) return 0;
+    return fail(ctx, "%s: the context is concat-conditioned (%d condition channels): call lfm_set_condition for exactly %d images "
+                     "first (the stored condition holds %d)", who, u->cond_ch, B_img, u->cond_rows);
+}
+
 extern "C" int lfm_forward(lfm_ctx* ctx, const float* t, int t_numel, const float* x, const int64_t* y, int B,
                            float cfg_scale, float* v_out, void* stream) {
     if (check_velocity_ready(ctx, B, "lfm_forward")) return 1;
@@ -787,9 +799,29 @@ extern "C" int lfm_forward(lfm_ctx* ctx, const float* t, int t_numel, const floa
     if (bind(ctx)) return 1;
     const bool cfg = cfg_scale > 1.0f;
     if (cfg && B % 2 != 0) return fail(ctx, "lfm_forward: forward_with_cfg needs an even batch (got %d)", B);
+    // a conditioned context takes x as the whole network input [B, in_channels, H, W] (WrapperCondFlow's cat([x, cond], 1))
+    const bool x_whole = ctx->un != nullptr && ctx->un->cond_ch > 0;
     // under CFG a vector t has 2n entries in the reference; both halves carry the same times (the x halves are identical)
     return eval_velocity(ctx, static_cast<cudaStream_t>(stream), t, t_numel, x, cfg ? B / 2 : B,
-                         reinterpret_cast<const long long*>(y), cfg_scale, 1, v_out);
+                         reinterpret_cast<const long long*>(y), cfg_scale, 1, v_out, x_whole);
+}
+
+extern "C" int lfm_set_condition(lfm_ctx* ctx, const float* cond, int B_img, int channels, void* stream) {
+    if (ctx == nullptr) return fail(ctx, "lfm_set_condition: null ctx");
+    if (ctx->net != NetKind::ADM || ctx->un->cond_ch == 0)
+        return fail(ctx, "lfm_set_condition: the context is not concat-conditioned (lfm_create_unet with in_channels > out_channels)");
+    UNetState* u = ctx->un;
+    if (channels != u->cond_ch)
+        return fail(ctx, "lfm_set_condition: channels must be in_channels - out_channels = %d (got %d)", u->cond_ch, channels);
+    if (!ctx->finalized) return fail(ctx, "lfm_set_condition: lfm_finalize has not been called");
+    if (B_img < 1 || B_img > ctx->max_rows)
+        return fail(ctx, "lfm_set_condition: B_img must be in [1, %d], the finalized rows (got %d)", ctx->max_rows, B_img);
+    if (cond == nullptr) return fail(ctx, "lfm_set_condition: cond must not be NULL");
+    if (bind(ctx)) return 1;
+    CUDA_OK(cudaMemcpyAsync(u->cond, cond, (size_t)B_img * channels * u->S * u->S * sizeof(float), cudaMemcpyDeviceToDevice,
+                            static_cast<cudaStream_t>(stream)));
+    u->cond_rows = B_img;
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -844,7 +876,7 @@ static int get_graph(lfm_ctx* ctx, const char* key, Record&& record, lfm_ctx::St
 // t_eval + j into k[j], and the update kernels read dt from the nodes ctx->t_grid.
 static int record_fixed_step(lfm_ctx* ctx, int method, int S, int n_img, bool has_y, float cfg_scale) {
     cudaStream_t s = ctx->stream;
-    const size_t n = (size_t)n_img * ctx->chw;
+    const size_t n = (size_t)n_img * ctx->out_chw;
     const long long* y = has_y ? ctx->y_buf : nullptr;
     const float* tg = ctx->t_grid;
     const StepState* st = ctx->step_state;
@@ -891,7 +923,7 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     const int perturb = (t_as_vector & LFM_FIXED_PERTURB) ? 1 : 0;
     if (perturb && method == LFM_METHOD_HEUN) return fail(ctx, "lfm_sample_fixed: perturb applies to the torchdiffeq grids (euler, midpoint, rk4)");
     const int rows = cfg_scale > 1.0f ? 2 * B_img : B_img;
-    if (check_velocity_ready(ctx, rows, "lfm_sample_fixed")) return 1;
+    if (check_velocity_ready(ctx, rows, "lfm_sample_fixed") || check_condition(ctx, B_img, "lfm_sample_fixed")) return 1;
     if (method < LFM_METHOD_EULER || method > LFM_METHOD_RK4) return fail(ctx, "lfm_sample_fixed: unknown method %d", method);
     if (n_grid < 2 || n_grid > 8192) return fail(ctx, "lfm_sample_fixed: n_grid must be in [2, 8192] (got %d)", n_grid);
     if (x_inout == nullptr || t_grid_host == nullptr) return fail(ctx, "lfm_sample_fixed: null tensor");
@@ -900,7 +932,7 @@ extern "C" int lfm_sample_fixed(lfm_ctx* ctx, int method, float* x_inout, const 
     if (method >= LFM_METHOD_MIDPOINT && n_int * S > 8192) return fail(ctx, "lfm_sample_fixed: too many stages (%d)", n_int * S);
     if (bind(ctx)) return 1;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
-    const size_t n = (size_t)B_img * ctx->chw;
+    const size_t n = (size_t)B_img * ctx->out_chw;
     const bool has_y = y != nullptr;
     if (join_in(ctx, user)) return 1;
     cudaStream_t s = ctx->stream;
@@ -1125,7 +1157,7 @@ extern "C" int lfm_sample_dopri5(lfm_ctx* ctx, float* x_inout, double t0, double
 extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, double t0, double t1, double rtol, double atol,
                                    const int64_t* y, int B_img, float cfg_scale, lfm_ode_stats* stats, void* stream) {
     const int rows = cfg_scale > 1.0f ? 2 * B_img : B_img;
-    if (check_velocity_ready(ctx, rows, "lfm_sample_adaptive")) return 1;
+    if (check_velocity_ready(ctx, rows, "lfm_sample_adaptive") || check_condition(ctx, B_img, "lfm_sample_adaptive")) return 1;
     if (method < LFM_ADAPTIVE_DOPRI5 || method > LFM_ADAPTIVE_HEUN) return fail(ctx, "lfm_sample_adaptive: unknown method %d", method);
     if (x_inout == nullptr) return fail(ctx, "lfm_sample_adaptive: null tensor");
     if (!(t0 > t1)) return fail(ctx, "lfm_sample_adaptive: expects t0 > t1 (reference integrates t: 1 -> 0)");
@@ -1133,7 +1165,7 @@ extern "C" int lfm_sample_adaptive(lfm_ctx* ctx, int method, float* x_inout, dou
     if (bind(ctx)) return 1;
     cudaStream_t user = static_cast<cudaStream_t>(stream);
     if (join_in(ctx, user)) return 1;
-    Dopri d{ctx, ctx->stream, B_img, nullptr, cfg_scale, (size_t)B_img * ctx->chw};
+    Dopri d{ctx, ctx->stream, B_img, nullptr, cfg_scale, (size_t)B_img * ctx->out_chw};
     d.tab = make_tableau(method);
     const RkTableau& tab = d.tab;
     const int ns = tab.n;
@@ -1424,6 +1456,29 @@ extern "C" int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const f
                                  int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
     return dbg_conv("lfm_dbg_conv_wide", true, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit,
                     stream);
+}
+
+// The network's conv_in (input_blocks.0 / conv_in) on the channel concatenation [a | b] of two NCHW fp32 sources.
+extern "C" int lfm_dbg_conv_in(const float* a, int a_ch, long long a_stride, const float* b, int b_ch, long long b_stride,
+                               const float* w, const float* bias, float* out, int B, int side, int Cout, void* stream) {
+    if (a_ch < 1 || b_ch < 0 || a_ch + b_ch < 3 || a_ch + b_ch > kConvInMaxChannels)
+        return fail(nullptr, "lfm_dbg_conv_in: a_ch >= 1, b_ch >= 0 and a_ch + b_ch in [3, %d] (got %d, %d)", kConvInMaxChannels, a_ch,
+                    b_ch);
+    if (side < 1 || side > 256 || conv_in_smem_bytes(a_ch + b_ch, side) > 48 * 1024)
+        return fail(nullptr, "lfm_dbg_conv_in: side must be in [1, 256] with a_ch + b_ch rows of side + 4 floats in 48 KB of shared "
+                             "memory (got side %d, %d channels)", side, a_ch + b_ch);
+    if (a_stride < (long long)a_ch * side * side || (b_ch > 0 && b_stride < (long long)b_ch * side * side))
+        return fail(nullptr, "lfm_dbg_conv_in: a_stride / b_stride must hold a_ch / b_ch channels of side^2 floats (got %lld, %lld)",
+                    a_stride, b_stride);
+    if (Cout < 1) return fail(nullptr, "lfm_dbg_conv_in: Cout must be >= 1 (got %d)", Cout);
+    if (B < 1 || (long long)B * side > INT32_MAX) return fail(nullptr, "lfm_dbg_conv_in: B must be >= 1 with B * side < 2^31 (got %d)", B);
+    if (a == nullptr || (b == nullptr) != (b_ch == 0) || w == nullptr || bias == nullptr || out == nullptr)
+        return fail(nullptr, "lfm_dbg_conv_in: a, w, bias and out must not be NULL, and b is NULL exactly when b_ch is 0");
+    return dbg_run([&](lfm_ctx* ctx) {
+        COUNT_LAUNCH(launch_conv_in(static_cast<cudaStream_t>(stream), ConvInSrc{a, a_ch, a_stride}, ConvInSrc{b, b_ch, b_stride}, B, B,
+                                    w, bias, out, side, Cout));
+        return 0;
+    });
 }
 
 extern "C" int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w_bf16, int w_rows, int w_ld, int K, int N,

@@ -267,39 +267,68 @@ gn_apply_bf16_kernel(GnApplyArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// input_blocks.0: conv3x3(in_channels=4 -> C), pad 1, NCHW fp32 latents -> NHWC fp32 stream (unet.py:464).
-// Network row b reads sample b % x_rows.  One block per output row (b, h); thread = output channel.
-__global__ void __launch_bounds__(256)
-conv_in_kernel(const float* __restrict__ x, int x_rows, const float* __restrict__ Wt /*[C,4,3,3]*/,
-               const float* __restrict__ bias, float* __restrict__ out, int H, int W, int C) {
-    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
-    pdl_trigger();
-    extern __shared__ float s_in[];  // [4][3][W + 2]
-    const int b = blockIdx.x / H, h = blockIdx.x % H;
-    const int bs = b % x_rows;
-    const int WP = W + 2;
-    for (int i = threadIdx.x; i < 4 * 3 * WP; i += blockDim.x) {
+// input_blocks.0: conv3x3(CIN -> C), pad 1, NCHW fp32 input -> NHWC fp32 stream (unet.py:464).  The CIN input channels are the
+// concatenation [a | b] of two NCHW fp32 sources (b.ch = 0: one source), so a concat-conditioned network (WrapperCondFlow:
+// model(t, cat([x, cond], 1))) reads the solver state and the condition where they lie.  Network row b reads image b % x_rows of
+// each source.  Every output sums from the bias in the order input channel -> filter row -> filter column; up to 36 weights per
+// thread (CIN <= 4) stay in registers, wider inputs are re-read per input channel.
+constexpr int kConvInMaxChannels = 16;
+struct ConvInSrc {
+    const float* p;
+    int ch;
+    long long img_stride;  // floats between two images
+};
+
+template <int CIN>
+__device__ __forceinline__ void conv_in_fill(float* s_in, ConvInSrc a, ConvInSrc b, int bs, int h, int H, int W, int WP) {
+    for (int i = threadIdx.x; i < CIN * 3 * WP; i += blockDim.x) {
         const int c = i / (3 * WP), r = (i / WP) % 3, w = i % WP - 1;
         const int hh = h + r - 1;
         float v = 0.f;
-        if (hh >= 0 && hh < H && w >= 0 && w < W) v = x[((static_cast<size_t>(bs) * 4 + c) * H + hh) * W + w];
+        if (hh >= 0 && hh < H && w >= 0 && w < W) {
+            const bool in_a = c < a.ch;
+            const float* p = in_a ? a.p : b.p;
+            const long long st = in_a ? a.img_stride : b.img_stride;
+            const int cs = in_a ? c : c - a.ch;
+            v = p[static_cast<size_t>(bs) * st + (static_cast<size_t>(cs) * H + hh) * W + w];
+        }
         s_in[i] = v;
     }
+}
+
+// One block per output row (b, h); thread = output channel.
+template <int CIN>
+__global__ void __launch_bounds__(256)
+conv_in_kernel(ConvInSrc a, ConvInSrc b, int x_rows, const float* __restrict__ Wt /*[C,CIN,3,3]*/,
+               const float* __restrict__ bias, float* __restrict__ out, int H, int W, int C) {
+    constexpr bool kRegW = CIN <= 4;
+    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
+    pdl_trigger();
+    extern __shared__ float s_in[];  // [CIN][3][W + 2]
+    const int b_ = blockIdx.x / H, h = blockIdx.x % H;
+    const int WP = W + 2;
+    conv_in_fill<CIN>(s_in, a, b, b_ % x_rows, h, H, W, WP);
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        float wreg[36];
+        const float* wc = Wt + static_cast<size_t>(c) * CIN * 9;
+        float wreg[kRegW ? CIN * 9 : 1];
+        if constexpr (kRegW) {
 #pragma unroll
-        for (int i = 0; i < 36; ++i) wreg[i] = __ldg(Wt + static_cast<size_t>(c) * 36 + i);
+            for (int i = 0; i < CIN * 9; ++i) wreg[i] = __ldg(wc + i);
+        }
         const float bc = bias[c];
         for (int w = 0; w < W; ++w) {
             float acc = bc;
 #pragma unroll
-            for (int ci = 0; ci < 4; ++ci)
+            for (int ci = 0; ci < CIN; ++ci)
 #pragma unroll
                 for (int r = 0; r < 3; ++r)
 #pragma unroll
-                    for (int s = 0; s < 3; ++s) acc = fmaf(wreg[ci * 9 + r * 3 + s], s_in[(ci * 3 + r) * WP + w + s], acc);
-            out[((static_cast<size_t>(b) * H + h) * W + w) * C + c] = acc;
+                    for (int s = 0; s < 3; ++s) {
+                        const float k = kRegW ? wreg[kRegW ? ci * 9 + r * 3 + s : 0] : __ldg(wc + ci * 9 + r * 3 + s);
+                        acc = fmaf(k, s_in[(ci * 3 + r) * WP + w + s], acc);
+                    }
+            out[((static_cast<size_t>(b_) * H + h) * W + w) * C + c] = acc;
         }
     }
 }
@@ -308,43 +337,47 @@ conv_in_kernel(const float* __restrict__ x, int x_rows, const float* __restrict_
 // (input channel, filter row) it fetches the 10 input values of the strip with three vector loads (warp-wide
 // broadcasts from shared memory) and issues 24 FMAs - 27 instructions per 8 outputs and tap row instead of 48.
 // Requires W % 8 == 0 (rows padded to W + 4 floats so that every strip starts 16-byte aligned).
+template <int CIN>
 __global__ void __launch_bounds__(256)
-conv_in_strip_kernel(const float* __restrict__ x, int x_rows, const float* __restrict__ Wt /*[C,4,3,3]*/,
+conv_in_strip_kernel(ConvInSrc a, ConvInSrc b, int x_rows, const float* __restrict__ Wt /*[C,CIN,3,3]*/,
                      const float* __restrict__ bias, float* __restrict__ out, int H, int W, int C) {
+    constexpr bool kRegW = CIN <= 4;
     pdl_wait();
     pdl_trigger();
-    extern __shared__ __align__(16) float s_in2[];  // [4][3][W + 4]: position p holds column p - 1
-    const int b = blockIdx.x / H, h = blockIdx.x % H;
-    const int bs = b % x_rows;
+    extern __shared__ __align__(16) float s_in2[];  // [CIN][3][W + 4]: position p holds column p - 1
+    const int b_ = blockIdx.x / H, h = blockIdx.x % H;
     const int WP = W + 4;
-    for (int i = threadIdx.x; i < 4 * 3 * WP; i += blockDim.x) {
-        const int c = i / (3 * WP), r = (i / WP) % 3, w = i % WP - 1;
-        const int hh = h + r - 1;
-        float v = 0.f;
-        if (hh >= 0 && hh < H && w >= 0 && w < W) v = x[((static_cast<size_t>(bs) * 4 + c) * H + hh) * W + w];
-        s_in2[i] = v;
-    }
+    conv_in_fill<CIN>(s_in2, a, b, b_ % x_rows, h, H, W, WP);
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        float wreg[36];
+        const float* wc = Wt + static_cast<size_t>(c) * CIN * 9;
+        float wreg[kRegW ? CIN * 9 : 1];
+        if constexpr (kRegW) {
 #pragma unroll
-        for (int i = 0; i < 36; ++i) wreg[i] = __ldg(Wt + static_cast<size_t>(c) * 36 + i);
+            for (int i = 0; i < CIN * 9; ++i) wreg[i] = __ldg(wc + i);
+        }
         const float bc = bias[c];
-        float* orow = out + (static_cast<size_t>(b) * H + h) * W * C + c;
+        float* orow = out + (static_cast<size_t>(b_) * H + h) * W * C + c;
         for (int w0 = 0; w0 < W; w0 += 8) {
             float acc[8];
 #pragma unroll
             for (int p = 0; p < 8; ++p) acc[p] = bc;
 #pragma unroll
-            for (int cr = 0; cr < 12; ++cr) {  // (input channel, filter row)
-                const float* ip = s_in2 + cr * WP + w0;
-                const float4 a0 = *reinterpret_cast<const float4*>(ip);
-                const float4 a1 = *reinterpret_cast<const float4*>(ip + 4);
-                const float2 a2 = *reinterpret_cast<const float2*>(ip + 8);
-                const float in[10] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y};
-                const float k0 = wreg[cr * 3], k1 = wreg[cr * 3 + 1], k2 = wreg[cr * 3 + 2];
+            for (int ci = 0; ci < CIN; ++ci) {
+                float k[9];
 #pragma unroll
-                for (int p = 0; p < 8; ++p) acc[p] = fmaf(k2, in[p + 2], fmaf(k1, in[p + 1], fmaf(k0, in[p], acc[p])));
+                for (int i = 0; i < 9; ++i) k[i] = kRegW ? wreg[kRegW ? ci * 9 + i : 0] : __ldg(wc + ci * 9 + i);
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {  // (input channel, filter row)
+                    const float* ip = s_in2 + (ci * 3 + r) * WP + w0;
+                    const float4 a0 = *reinterpret_cast<const float4*>(ip);
+                    const float4 a1 = *reinterpret_cast<const float4*>(ip + 4);
+                    const float2 a2 = *reinterpret_cast<const float2*>(ip + 8);
+                    const float in[10] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y};
+                    const float k0 = k[r * 3], k1 = k[r * 3 + 1], k2 = k[r * 3 + 2];
+#pragma unroll
+                    for (int p = 0; p < 8; ++p) acc[p] = fmaf(k2, in[p + 2], fmaf(k1, in[p + 1], fmaf(k0, in[p], acc[p])));
+                }
             }
 #pragma unroll
             for (int p = 0; p < 8; ++p) orow[static_cast<size_t>(w0 + p) * C] = acc[p];

@@ -171,7 +171,7 @@ class _NativeNet(nn.Module):
     def _forward_native(self, t, x, y, cfg_scale=1.0):
         B = x.shape[0]
         ctx = self.native(B, x.device)
-        v = torch.empty_like(x)
+        v = x.new_empty((B, self.out_channels) + tuple(x.shape[2:]))
         _lib.check(_lib.load().lfm_forward(ctx, t.data_ptr(), t.numel(), x.data_ptr(), y.data_ptr() if y is not None else None,
                                            B, float(cfg_scale), v.data_ptr(), self._stream(x.device)), ctx)
         return v

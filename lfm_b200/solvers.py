@@ -30,13 +30,41 @@ HEUN_REFERENCE_CORRECTOR_LIMIT = 39
 
 
 def _unwrap(model):
-    """Accept the NFECount-style wrappers of the reference CLI (attribute .model)."""
+    """Accept the NFECount-style wrappers of the reference CLI and the downstream tasks' WrapperCondFlow (attribute .model;
+    _condition reads the latter's .cond)."""
     inner = model
     while not isinstance(inner, _NativeNet) and hasattr(inner, "model"):
         inner = inner.model
     if not isinstance(inner, _NativeNet):
         raise TypeError("lfm_b200 solvers need an lfm_b200 network (got %r)" % type(model).__name__)
     return inner
+
+
+def _condition(model):
+    """The condition a chain of WrapperCondFlow-style wrappers (attribute .cond) concatenates to the state: the wrapper
+    nearest the caller concatenates first, so the network sees cat([x, cond_outer, ..., cond_inner], 1).  None without one."""
+    conds = []
+    inner = model
+    while not isinstance(inner, _NativeNet) and hasattr(inner, "model"):
+        if getattr(inner, "cond", None) is not None:
+            conds.append(inner.cond)
+        inner = inner.model
+    return torch.cat(conds, 1) if conds else None
+
+
+def _set_condition(net, ctx, cond, x):
+    """Hand the wrapper chain's condition to a concat-conditioned network (lfm_set_condition) before a native sampler runs."""
+    n_cond = net.in_channels - net.out_channels
+    if cond is None:
+        if n_cond:
+            raise ValueError(f"the network takes {net.in_channels} input channels: wrap it in WrapperCondFlow(model, cond) with "
+                             f"a {n_cond}-channel condition")
+        return
+    if cond.dim() != 4 or cond.shape[0] != x.shape[0] or cond.shape[2:] != x.shape[2:] or cond.shape[1] != n_cond:
+        raise ValueError(f"the condition must be [{x.shape[0]}, {n_cond}, {x.shape[2]}, {x.shape[3]}] for this network and state "
+                         f"(got {tuple(cond.shape)})")
+    cond = cond.to(device=x.device, dtype=torch.float32).contiguous()
+    _lib.check(_lib.load().lfm_set_condition(ctx, cond.data_ptr(), x.shape[0], n_cond, _NativeNet._stream(x.device)), ctx)
 
 
 def _split_cfg(x, model_kwargs):
@@ -78,6 +106,7 @@ def _run_native(model, x, y, cfg_scale, entry, method, *args):
     rows = 2 * n_img if cfg_scale > 1.0 else n_img
     y = _check_labels(net, y, rows, x.device)
     ctx = net.native(rows, x.device)
+    _set_condition(net, ctx, _condition(model), x)
     stats = _lib.OdeStats()
     _lib.check(getattr(_lib.load(), entry)(
         ctx, method, x.data_ptr(), *args, y.data_ptr() if y is not None else None, n_img, float(cfg_scale), C.byref(stats),

@@ -127,4 +127,6 @@ class UNetModel(_NativeNet):
         assert (y is not None) == (self.num_classes is not None), \
             "must specify y if and only if the model is class-conditional"
         t, x, y, B = self._prep(timesteps, x, y)
+        if x.dim() != 4 or x.shape[1] != self.in_channels:
+            raise ValueError(f"x must be [B, {self.in_channels}, H, W] (got {tuple(x.shape)})")
         return self._forward_native(t, x, y)
