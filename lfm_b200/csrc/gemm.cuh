@@ -186,6 +186,101 @@ LFM_DEVICE void gn_add(unsigned long long* bins_b, int g, float s, float q) {
     atomicAdd(bins_b + 2 * g + 1, static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(q) * kGnFixScaleSq)));
 }
 
+// 4 x 4 transpose of 32-bit items within each quad of lanes (q = lane % 4): a[i] of lane q becomes a[q] of lane i.
+LFM_DEVICE void quad_transpose(uint32_t (&a)[4]) {
+    const int lane = threadIdx.x & 31, q = lane & 3;
+    uint32_t b[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) b[s] = (s == q) ? a[s] : 0u;
+#pragma unroll
+    for (int k = 1; k < 4; ++k) {
+        const int send = (q + k) & 3, from = (q - k) & 3;  // lane q sends its item for lane q + k, receives from lane q - k
+        const uint32_t v = send == 0 ? a[0] : send == 1 ? a[1] : send == 2 ? a[2] : a[3];
+        const uint32_t r = __shfl_sync(0xffffffffu, v, (lane & ~3) | from);
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+            if (s == from) b[s] = r;
+    }
+#pragma unroll
+    for (int s = 0; s < 4; ++s) a[s] = b[s];
+}
+
+// Epilogue of 32 whole columns c32 .. c32 + 31 (in range, 16-byte aligned rows) from acc[0, 16) of the accumulator layout:
+// the same arithmetic per element as the per-8-column path, then a quad transpose so that lane q holds columns
+// c32 + 8 q .. + 7 of its two rows and stores them with 16-byte accesses.
+template <int EPI>
+LFM_DEVICE void epilogue_store_32(const float* acc, const GemmEpi& ep, int c32, bool ok0, bool ok1, int row0, int row1, int orow0,
+                                  int orow1, const float* gate0, const float* gate1) {
+    const int q = threadIdx.x & 3;
+    uint32_t r0a[4], r0b[4], r1a[4], r1b[4];  // bf16: packed pairs in r0a / r1a; fp32: .x in *a, .y in *b
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int col = c32 + 8 * k + 2 * q;
+        float v0 = acc[4 * k], v1 = acc[4 * k + 1], v2 = acc[4 * k + 2], v3 = acc[4 * k + 3];
+        if (ep.bias != nullptr) {
+            const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
+            v0 += b0, v1 += b1, v2 += b0, v3 += b1;
+        }
+        if (EPI == EPI_BIAS_GELU_BF16) {
+            v0 = gelu_tanh(v0), v1 = gelu_tanh(v1), v2 = gelu_tanh(v2), v3 = gelu_tanh(v3);
+        }
+        if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16) {
+            r0a[k] = pack_bf16x2(v0, v1);
+            r1a[k] = pack_bf16x2(v2, v3);
+        } else {
+            r0a[k] = __float_as_uint(v0), r0b[k] = __float_as_uint(v1);
+            r1a[k] = __float_as_uint(v2), r1b[k] = __float_as_uint(v3);
+        }
+    }
+    const int col = c32 + 8 * q;  // this lane's 8 columns after the transpose; item p = columns col + 2 p, + 1
+    if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16) {
+        quad_transpose(r0a);
+        quad_transpose(r1a);
+        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(ep.out);
+        if (ok0) *reinterpret_cast<uint4*>(o + static_cast<size_t>(orow0) * ep.ldo + col) = make_uint4(r0a[0], r0a[1], r0a[2], r0a[3]);
+        if (ok1) *reinterpret_cast<uint4*>(o + static_cast<size_t>(orow1) * ep.ldo + col) = make_uint4(r1a[0], r1a[1], r1a[2], r1a[3]);
+        return;
+    }
+    quad_transpose(r0a);
+    quad_transpose(r0b);
+    quad_transpose(r1a);
+    quad_transpose(r1b);
+    float* o = static_cast<float*>(ep.out);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const bool ok = h == 0 ? ok0 : ok1;
+        if (!ok) continue;
+        const uint32_t* ra = h == 0 ? r0a : r1a;
+        const uint32_t* rb = h == 0 ? r0b : r1b;
+        float v[8];
+#pragma unroll
+        for (int p = 0; p < 4; ++p) v[2 * p] = __uint_as_float(ra[p]), v[2 * p + 1] = __uint_as_float(rb[p]);
+        if (EPI == EPI_BIAS_F32) {
+            float4* d = reinterpret_cast<float4*>(o + static_cast<size_t>(h == 0 ? orow0 : orow1) * ep.ldo + col);
+            d[0] = make_float4(v[0], v[1], v[2], v[3]);
+            d[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {  // EPI_GATE_RESID_F32
+            float4* d = reinterpret_cast<float4*>(o + static_cast<size_t>(h == 0 ? row0 : row1) * ep.ldo + col);
+            const float* g = h == 0 ? gate0 : gate1;
+            float4 x0 = d[0], x1 = d[1];
+            float* x = reinterpret_cast<float*>(&x0);
+            float* y = reinterpret_cast<float*>(&x1);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (g != nullptr) {
+                    x[j] = fmaf(__ldg(g + col + j), v[j], x[j]);
+                    y[j] = fmaf(__ldg(g + col + 4 + j), v[4 + j], y[j]);
+                } else {
+                    x[j] += v[j];
+                    y[j] += v[4 + j];
+                }
+            }
+            d[0] = x0;
+            d[1] = x1;
+        }
+    }
+}
+
 // Work items: (tile, k-slice).  ksplit > 1 (split-K, for GEMMs with far fewer tiles than SMs): every slice stores its fp32
 // partial tile, without bias, into its own slab of ep.out (row offset slice * split_row_pitch); a separate kernel adds the
 // slabs in a fixed order.
@@ -343,70 +438,83 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 bins_b = ep.gn_bins + (static_cast<size_t>(wrow / ep.gn_hw) * kGnBinReplicas + rep) * 64;
             }
             float gs = 0.f, gq = 0.f;
+            // Whole 32-column groups are stored 16 bytes per lane (a quad of lanes writes 64 contiguous bytes of a row, 128 for
+            // fp32) after a transpose within the quad; the per-8-column path below takes the N tail, the GroupNorm statistics and
+            // rows whose pitch or base is not 16-byte aligned.
+            const bool vec = !gn && ep.ldo % 8 == 0 && (reinterpret_cast<uintptr_t>(ep.out) & 15) == 0;
 #pragma unroll
-            for (int i = 0; i < BN / 8; ++i) {
-                const int c8 = nbase + 8 * i;  // warp-uniform
-                if (c8 >= N) break;
-                const int col = c8 + 2 * (lane & 3);
-                const bool cok = col < N;  // N is even; a tail narrower than 8 columns (N = 4) ends inside the block
-                const bool w0 = ok0 && cok, w1 = ok1 && cok;
-                float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
-                if (ep.bias != nullptr && cok) {
-                    const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
-                    v0 += b0, v1 += b1, v2 += b0, v3 += b1;
+            for (int i4 = 0; i4 < BN / 8; i4 += 4) {
+                const int c32 = nbase + 8 * i4;  // warp-uniform
+                if (c32 >= N) break;
+                if (vec && c32 + 32 <= N) {
+                    epilogue_store_32<EPI>(acc + 4 * i4, ep, c32, ok0, ok1, row0, row1, orow0, orow1, gate0, gate1);
+                    continue;
                 }
-                if (EPI == EPI_BIAS_GELU_BF16) {
-                    v0 = gelu_tanh(v0), v1 = gelu_tanh(v1), v2 = gelu_tanh(v2), v3 = gelu_tanh(v3);
-                }
-                if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16) {
-                    __nv_bfloat16* o = static_cast<__nv_bfloat16*>(ep.out);
-                    if (w0) *reinterpret_cast<uint32_t*>(o + static_cast<size_t>(orow0) * ep.ldo + col) = pack_bf16x2(v0, v1);
-                    if (w1) *reinterpret_cast<uint32_t*>(o + static_cast<size_t>(orow1) * ep.ldo + col) = pack_bf16x2(v2, v3);
-                } else if (EPI == EPI_BIAS_F32) {
-                    float* o = static_cast<float*>(ep.out);
-                    if (w0) *reinterpret_cast<float2*>(o + static_cast<size_t>(orow0) * ep.ldo + col) = make_float2(v0, v1);
-                    if (w1) *reinterpret_cast<float2*>(o + static_cast<size_t>(orow1) * ep.ldo + col) = make_float2(v2, v3);
-                } else {  // EPI_GATE_RESID_F32
-                    float* o = static_cast<float*>(ep.out);
-                    if (w0) {
-                        float2* p = reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * ep.ldo + col);
-                        float2 x = *p;
-                        if (gate0 != nullptr) {
-                            x.x = fmaf(__ldg(gate0 + col), v0, x.x);
-                            x.y = fmaf(__ldg(gate0 + col + 1), v1, x.y);
-                        } else {
-                            x.x += v0, x.y += v1;
-                        }
-                        *p = x;
+#pragma unroll
+                for (int i = i4; i < i4 + 4; ++i) {
+                    const int c8 = nbase + 8 * i;  // warp-uniform
+                    if (c8 >= N) break;
+                    const int col = c8 + 2 * (lane & 3);
+                    const bool cok = col < N;  // N is even; a tail narrower than 8 columns (N = 4) ends inside the block
+                    const bool w0 = ok0 && cok, w1 = ok1 && cok;
+                    float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
+                    if (ep.bias != nullptr && cok) {
+                        const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
+                        v0 += b0, v1 += b1, v2 += b0, v3 += b1;
                     }
-                    if (w1) {
-                        float2* p = reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * ep.ldo + col);
-                        float2 x = *p;
-                        if (gate1 != nullptr) {
-                            x.x = fmaf(__ldg(gate1 + col), v2, x.x);
-                            x.y = fmaf(__ldg(gate1 + col + 1), v3, x.y);
-                        } else {
-                            x.x += v2, x.y += v3;
-                        }
-                        *p = x;
+                    if (EPI == EPI_BIAS_GELU_BF16) {
+                        v0 = gelu_tanh(v0), v1 = gelu_tanh(v1), v2 = gelu_tanh(v2), v3 = gelu_tanh(v3);
                     }
-                }
-                if (EPI == EPI_BIAS_F32 || EPI == EPI_BIAS_BF16) {
-                    if (gn) {  // warp-uniform
-                        if (!w0) v0 = v1 = 0.f;
-                        if (!w1) v2 = v3 = 0.f;
-                        gs += (v0 + v1) + (v2 + v3);
-                        gq += (v0 * v0 + v1 * v1) + (v2 * v2 + v3 * v3);
-                        if (ep.gn_cpg == 4) {
-                            // two groups in these 8 columns: lanes with lane % 4 in {0, 1} hold group 2 i, {2, 3} group 2 i + 1
-                            const float s4 = warp_sum_mask(gs, 4), q4 = warp_sum_mask(gq, 4);
-                            const float s = s4 + __shfl_xor_sync(0xffffffffu, s4, 1), q = q4 + __shfl_xor_sync(0xffffffffu, q4, 1);
-                            if ((lane & ~2) == 0) gn_add(bins_b, col / 4, s, q);
-                            gs = gq = 0.f;
-                        } else if (((8 * (i + 1)) % ep.gn_cpg) == 0) {  // last 8 columns of a group
-                            const float s = warp_sum_mask(gs, 1), q = warp_sum_mask(gq, 1);
-                            if (lane == 0) gn_add(bins_b, c8 / ep.gn_cpg, s, q);
-                            gs = gq = 0.f;
+                    if (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16) {
+                        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(ep.out);
+                        if (w0) *reinterpret_cast<uint32_t*>(o + static_cast<size_t>(orow0) * ep.ldo + col) = pack_bf16x2(v0, v1);
+                        if (w1) *reinterpret_cast<uint32_t*>(o + static_cast<size_t>(orow1) * ep.ldo + col) = pack_bf16x2(v2, v3);
+                    } else if (EPI == EPI_BIAS_F32) {
+                        float* o = static_cast<float*>(ep.out);
+                        if (w0) *reinterpret_cast<float2*>(o + static_cast<size_t>(orow0) * ep.ldo + col) = make_float2(v0, v1);
+                        if (w1) *reinterpret_cast<float2*>(o + static_cast<size_t>(orow1) * ep.ldo + col) = make_float2(v2, v3);
+                    } else {  // EPI_GATE_RESID_F32
+                        float* o = static_cast<float*>(ep.out);
+                        if (w0) {
+                            float2* p = reinterpret_cast<float2*>(o + static_cast<size_t>(row0) * ep.ldo + col);
+                            float2 x = *p;
+                            if (gate0 != nullptr) {
+                                x.x = fmaf(__ldg(gate0 + col), v0, x.x);
+                                x.y = fmaf(__ldg(gate0 + col + 1), v1, x.y);
+                            } else {
+                                x.x += v0, x.y += v1;
+                            }
+                            *p = x;
+                        }
+                        if (w1) {
+                            float2* p = reinterpret_cast<float2*>(o + static_cast<size_t>(row1) * ep.ldo + col);
+                            float2 x = *p;
+                            if (gate1 != nullptr) {
+                                x.x = fmaf(__ldg(gate1 + col), v2, x.x);
+                                x.y = fmaf(__ldg(gate1 + col + 1), v3, x.y);
+                            } else {
+                                x.x += v2, x.y += v3;
+                            }
+                            *p = x;
+                        }
+                    }
+                    if (EPI == EPI_BIAS_F32 || EPI == EPI_BIAS_BF16) {
+                        if (gn) {  // warp-uniform
+                            if (!w0) v0 = v1 = 0.f;
+                            if (!w1) v2 = v3 = 0.f;
+                            gs += (v0 + v1) + (v2 + v3);
+                            gq += (v0 * v0 + v1 * v1) + (v2 * v2 + v3 * v3);
+                            if (ep.gn_cpg == 4) {
+                                // two groups in these 8 columns: lanes with lane % 4 in {0, 1} hold group 2 i, {2, 3} group 2 i + 1
+                                const float s4 = warp_sum_mask(gs, 4), q4 = warp_sum_mask(gq, 4);
+                                const float s = s4 + __shfl_xor_sync(0xffffffffu, s4, 1), q = q4 + __shfl_xor_sync(0xffffffffu, q4, 1);
+                                if ((lane & ~2) == 0) gn_add(bins_b, col / 4, s, q);
+                                gs = gq = 0.f;
+                            } else if (((8 * (i + 1)) % ep.gn_cpg) == 0) {  // last 8 columns of a group
+                                const float s = warp_sum_mask(gs, 1), q = warp_sum_mask(gq, 1);
+                                if (lane == 0) gn_add(bins_b, c8 / ep.gn_cpg, s, q);
+                                gs = gq = 0.f;
+                            }
                         }
                     }
                 }
