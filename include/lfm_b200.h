@@ -203,6 +203,33 @@ int64_t lfm_launch_count(const lfm_ctx* ctx);
  * pick for this shape; any other value is rejected. */
 int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
                  int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream);
+/* lfm_dbg_gemm with the persistent tile loop walking the 128-row blocks from the last to the first (the network sets this on
+ * every other GEMM); same arguments and results. */
+int lfm_dbg_gemm_reversed(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                          int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream);
+/* The DiT's LayerNorm (no affine, eps 1e-6) + adaLN modulate: y[r] = bf16((x[r] - mean) rstd (1 + scale[b]) + shift[b]),
+ * b = r / rows_per_sample, the vectors of sample b at shift / scale + b * mod_stride (0: one shared row).  x fp32 [M, D],
+ * y bf16 [M, D].  D = 128 x {2, 3, 6, 8, 9}; rows_per_sample a multiple of 16; down 1 sweeps the rows downwards.  All pointers
+ * 16-byte aligned, mod_stride a multiple of 4. */
+int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* shift, const float* scale, int mod_stride, int rows_per_sample,
+                        int M, int D, int down, void* stream);
+/* The DiT's conditioning for `rows` rows, each stage into a caller-allocated output: tf_out fp32 [rows, 256] timestep features
+ * [cos | sin] of t (t_numel 1 or rows), h1_out fp32 [rows, D] = SiLU(w0 tf + b0), c_bf16 bf16 [rows, D] =
+ * SiLU(w2 h1 + b2 + table[y[r]]), y NULL = the null row table_rows - 1 for every row.  w0 [D, 256], w2 [D, D], table
+ * [table_rows, D], all fp32; D a multiple of 128 up to 1152. */
+int lfm_dbg_dit_condition(const float* t, int t_numel, const long long* y, int rows, int D, const float* w0, const float* b0,
+                          const float* w2, const float* b2, const float* table, int table_rows, float* tf_out, float* h1_out,
+                          void* c_bf16, void* stream);
+/* The DiT's patch embed: M token rows of G x G tokens per sample, row m of sample b = m / G^2 reads latent b % x_rows of x (NCHW
+ * fp32, C channels of side p G).  Wt fp32 [C p p, D] (the conv weight transposed, patch vector order (c, p, q)), bias [D],
+ * pos [G^2, D] -> tok fp32 [M, D].  p 2 (C 4), 4 or 8; D a multiple of 4. */
+int lfm_dbg_patch_embed(const float* x, int x_rows, const float* Wt, const float* bias, const float* pos, float* tok, int D, int G,
+                        int C, int p, int M, void* stream);
+/* The DiT's FinalLayer (LayerNorm, modulate with shift / scale + b * mod_stride, Linear(D, p p C)) and unpatchify: x fp32 [M, D]
+ * -> v_net fp32 NCHW [M / G^2, C, p G, p G].  W fp32 [p p C, D] with out-feature (pp p + q) C + c, bias [p p C].  p 2 (C 4), 4 or
+ * 8; D a multiple of 128 up to 1536; mod_stride a multiple of 4. */
+int lfm_dbg_final_layer(const float* x, const float* shift, const float* scale, int mod_stride, const float* W, const float* bias,
+                        float* v_net, int M, int D, int G, int C, int p, void* stream);
 /* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer in the timm feature order ({q,k,v} * D + head * 64 + c) -> out [B*256, D]
  * bf16.  variant 0: the TMA + wgmma kernel the network runs for 256 tokens; 1: the mma.sync flash kernel.  dbg_s must be NULL. */
 int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s, void* stream);

@@ -651,6 +651,51 @@ static int check_ready(lfm_ctx* ctx, int rows, const char* who);
 #include "unet_host.inc"
 #include "vae_host.inc"
 
+// The DiT's conditioning for `rows` rows (models/DiT.py:125,264): tf = timestep features of t (t_numel 1 broadcasts),
+// h1 = SiLU(mlp.0(tf)) (fp32), c = SiLU(mlp.2(h1) + table[y]) (bf16, the adaLN GEMM's operand).  y NULL reads the null row
+// table_rows - 1.  w0 [D, 256], w2 [D, D]: D / 128 <= 9 float4 per lane (skinny_linear_kernel).
+static int launch_dit_condition(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const long long* y, int rows, int D,
+                                const float* w0, const float* b0, const float* w2, const float* b2, const float* table,
+                                int table_rows, float* tf, float* h1, __nv_bfloat16* c) {
+    timestep_features_kernel<<<rows, 256, 0, s>>>(t, t_numel, tf, rows);
+    LAUNCH_OK();
+    skinny_linear_kernel<0><<<(D + 7) / 8, 256, 0, s>>>(w0, b0, tf, rows, D, 256, nullptr, nullptr, 0, h1, nullptr);
+    LAUNCH_OK();
+    skinny_linear_kernel<1><<<(D + 7) / 8, 256, 0, s>>>(w2, b2, h1, rows, D, D, table, y, table_rows - 1, nullptr, c);
+    LAUNCH_OK();
+    return 0;
+}
+
+// Patch embed of M token rows (T = G^2 per sample; row b reads latent b % x_rows): the specialised kernel for p = 2 (C = 4),
+// the generic one, with its 8 patch vectors in dynamic shared memory, for p = 4 and 8.
+static int launch_patch_embed(lfm_ctx* ctx, cudaStream_t s, const float* x, int x_rows, const float* Wt, const float* bias,
+                              const float* pos, float* tok, int D, int G, int C, int p, int M) {
+    if (p == 2) {
+        patch_embed_kernel<<<(M + 7) / 8, 256, 0, s>>>(x, x_rows, Wt, bias, pos, tok, D, G, C, M);
+    } else {
+        const int smem = 8 * C * p * p * (int)sizeof(float);
+        patch_embed_generic_kernel<<<(M + 7) / 8, 256, smem, s>>>(x, x_rows, Wt, bias, pos, tok, D, G, C, p, M);
+    }
+    LAUNCH_OK();
+    return 0;
+}
+
+// FinalLayer + unpatchify of M token rows into v_net (NCHW fp32): the specialised kernel (16 x D weight in shared memory) for
+// p = 2 (C = 4), the generic one for p = 4 and 8.  At most 2 blocks per SM; each warp loops over the rows beyond.
+static int launch_final_layer(lfm_ctx* ctx, cudaStream_t s, const float* x, const float* shift, const float* scale, int mod_stride,
+                              const float* W, const float* bias, float* v_net, int M, int D, int G, int C, int p) {
+    static DevOnce once;
+    CUDA_OK(smem_opt_in(once, final_layer_kernel, 16 * 1536 * 4));  // largest supported width (hidden_size <= 1536)
+    int grid = (M + 7) / 8;
+    if (grid > 2 * g_num_sms) grid = 2 * g_num_sms;
+    if (p == 2)
+        final_layer_kernel<<<grid, 256, 16 * D * (int)sizeof(float), s>>>(x, shift, scale, mod_stride, W, bias, v_net, M, D, G, C);
+    else
+        final_layer_generic_kernel<<<grid, 256, 0, s>>>(x, shift, scale, mod_stride, W, bias, v_net, M, D, G, C, p);
+    LAUNCH_OK();
+    return 0;
+}
+
 // x_whole: see run_unet_program (conditioned UNets only)
 static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const float* x, int x_rows,
                           const long long* y, int rows, bool x_whole) {
@@ -662,28 +707,15 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     const bool uniform_c = (t_numel == 1 && y == nullptr);
     const int crows = uniform_c ? 1 : rows;
     const int Nmod = uniform_c ? 0 : ctx->Nmod;  // stride between samples in the modulation table
-    timestep_features_kernel<<<crows, 256, 0, s>>>(t, t_numel, ctx->tfreq, crows);
-    LAUNCH_OK();
-    skinny_linear_kernel<0><<<(D + 7) / 8, 256, 0, s>>>(ctx->t_w0, ctx->t_b0, ctx->tfreq, crows, D, 256, nullptr, nullptr,
-                                                        0, ctx->h1, nullptr);
-    LAUNCH_OK();
-    skinny_linear_kernel<1><<<(D + 7) / 8, 256, 0, s>>>(ctx->t_w2, ctx->t_b2, ctx->h1, crows, D, D, ctx->ytable, y,
-                                                        ctx->d.table_rows - 1, nullptr, ctx->c_silu);
-    LAUNCH_OK();
+    if (launch_dit_condition(ctx, s, t, t_numel, y, crows, D, ctx->t_w0, ctx->t_b0, ctx->t_w2, ctx->t_b2, ctx->ytable,
+                             ctx->d.table_rows, ctx->tfreq, ctx->h1, ctx->c_silu))
+        return 1;
     {   // all adaLN modulation vectors of the network in one GEMM: mod[crows, (6L+2) D]
         GemmEpi ep{ctx->b_mod, ctx->mod, ctx->Nmod, nullptr, 0, 1};
         COUNT_LAUNCH(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
     }
     const int ps = ctx->d.patch_size;
-    if (ps == 2) {
-        patch_embed_kernel<<<(M + 7) / 8, 256, 0, s>>>(x, x_rows, ctx->pe_w, ctx->pe_b, ctx->pos, ctx->x_tok, D, ctx->G,
-                                                       ctx->C, M);
-    } else {
-        const int smem = 8 * ctx->C * ps * ps * (int)sizeof(float);
-        patch_embed_generic_kernel<<<(M + 7) / 8, 256, smem, s>>>(x, x_rows, ctx->pe_w, ctx->pe_b, ctx->pos, ctx->x_tok, D,
-                                                                  ctx->G, ctx->C, ps, M);
-    }
-    LAUNCH_OK();
+    if (launch_patch_embed(ctx, s, x, x_rows, ctx->pe_w, ctx->pe_b, ctx->pos, ctx->x_tok, D, ctx->G, ctx->C, ps, M)) return 1;
     // L2 zig-zag: consecutive kernels sweep the token rows in opposite directions, so each starts on the rows its
     // producer wrote last (still L2-resident) instead of the rows that were evicted first.
     int dir = 1;  // patch_embed wrote x_tok upwards
@@ -729,22 +761,8 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
         }
     }
-    {
-        const float* mf = ctx->mod + (size_t)6 * L * D;  // shift | scale
-        static DevOnce once;
-        const int smem = 16 * D * (int)sizeof(float);
-        CUDA_OK(smem_opt_in(once, final_layer_kernel, 16 * 1536 * 4));  // largest supported width (hidden_size <= 1536)
-        int grid = (M + 7) / 8;
-        if (grid > 2 * g_num_sms) grid = 2 * g_num_sms;
-        if (ps == 2)
-            final_layer_kernel<<<grid, 256, smem, s>>>(ctx->x_tok, mf, mf + D, Nmod, ctx->fin_w, ctx->fin_b, ctx->v_net, M, D,
-                                                       ctx->G, ctx->C);
-        else
-            final_layer_generic_kernel<<<grid, 256, 0, s>>>(ctx->x_tok, mf, mf + D, Nmod, ctx->fin_w, ctx->fin_b, ctx->v_net, M,
-                                                            D, ctx->G, ctx->C, ps);
-        LAUNCH_OK();
-    }
-    return 0;
+    const float* mf = ctx->mod + (size_t)6 * L * D;  // shift | scale
+    return launch_final_layer(ctx, s, ctx->x_tok, mf, mf + D, Nmod, ctx->fin_w, ctx->fin_b, ctx->v_net, M, D, ctx->G, ctx->C, ps);
 }
 
 // Evaluate the (CFG-combined) velocity of n_img latents in `x` into `v_out` [n_img, C, H, W].
@@ -1319,20 +1337,112 @@ static int dbg_run(Op&& op) {
     return op(&dbg);
 }
 
-extern "C" int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
-                            int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n,
-                            void* stream) {
-    if (K % 64 != 0 || N % 8 != 0) return fail(nullptr, "lfm_dbg_gemm: K must be a multiple of 64 and N of 8");
-    if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(nullptr, "lfm_dbg_gemm: unknown epilogue %d", epi);
+// lfm_dbg_gemm and lfm_dbg_gemm_reversed: `reverse` sets GemmEpi::reverse_m, as the network does on every other GEMM.
+static int dbg_gemm(const char* who, int reverse, const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                    int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream) {
+    if (K % 64 != 0 || N % 8 != 0) return fail(nullptr, "%s: K must be a multiple of 64 and N of 8", who);
+    if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(nullptr, "%s: unknown epilogue %d", who, epi);
     if (block_n != 0 && block_n != 128 && block_n != 256)
-        return fail(nullptr, "lfm_dbg_gemm: block_n must be 0, 128 or 256 (got %d)", block_n);
+        return fail(nullptr, "%s: block_n must be 0, 128 or 256 (got %d)", who, block_n);
     return dbg_run([&](lfm_ctx* ctx) {
         CUtensorMap ta, tb;
         if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
-            return fail(ctx, "lfm_dbg_gemm: tensor map encode failed");
+            return fail(ctx, "%s: tensor map encode failed", who);
         GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
+        ep.reverse_m = reverse;
         CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
         return 0;
+    });
+}
+
+extern "C" int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                            int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n,
+                            void* stream) {
+    return dbg_gemm("lfm_dbg_gemm", 0, a_bf16, w_bf16, bias, out, gate, gate_stride, rows_per_sample, M, N, K, epi, block_n, stream);
+}
+
+extern "C" int lfm_dbg_gemm_reversed(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                                     int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n,
+                                     void* stream) {
+    return dbg_gemm("lfm_dbg_gemm_reversed", 1, a_bf16, w_bf16, bias, out, gate, gate_stride, rows_per_sample, M, N, K, epi, block_n,
+                    stream);
+}
+
+// The DiT's own kernels, each through the helper launch_network calls.
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+extern "C" int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* shift, const float* scale, int mod_stride,
+                                   int rows_per_sample, int M, int D, int down, void* stream) {
+    const int nv = D / 128;
+    if (D % 128 != 0 || !(nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9))
+        return fail(nullptr, "lfm_dbg_ln_modulate: D must be 128 x {2, 3, 6, 8, 9} (got %d)", D);
+    if (rows_per_sample < kLnRows || rows_per_sample % kLnRows != 0)
+        return fail(nullptr, "lfm_dbg_ln_modulate: rows_per_sample must be a positive multiple of %d (got %d)", kLnRows, rows_per_sample);
+    if (M < 1) return fail(nullptr, "lfm_dbg_ln_modulate: M must be >= 1 (got %d)", M);
+    if (mod_stride < 0 || mod_stride % 4 != 0)
+        return fail(nullptr, "lfm_dbg_ln_modulate: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
+    if (down != 0 && down != 1) return fail(nullptr, "lfm_dbg_ln_modulate: down must be 0 or 1 (got %d)", down);
+    if (!aligned16(x) || !aligned16(shift) || !aligned16(scale) || !aligned16(y_bf16) || x == nullptr || y_bf16 == nullptr ||
+        shift == nullptr || scale == nullptr)
+        return fail(nullptr, "lfm_dbg_ln_modulate: x, y, shift and scale must not be NULL and must be 16-byte aligned");
+    return dbg_run([&](lfm_ctx* ctx) {
+        COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<__nv_bfloat16*>(y_bf16), shift, scale, mod_stride,
+                               rows_per_sample, M, D, down));
+        return 0;
+    });
+}
+
+extern "C" int lfm_dbg_dit_condition(const float* t, int t_numel, const long long* y, int rows, int D, const float* w0, const float* b0,
+                                     const float* w2, const float* b2, const float* table, int table_rows, float* tf_out, float* h1_out,
+                                     void* c_bf16, void* stream) {
+    if (rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: rows must be >= 1 (got %d)", rows);
+    if (t_numel != 1 && t_numel != rows)
+        return fail(nullptr, "lfm_dbg_dit_condition: t_numel must be 1 or rows (got %d, rows %d)", t_numel, rows);
+    if (D < 128 || D % 128 != 0 || D > 9 * 128)
+        return fail(nullptr, "lfm_dbg_dit_condition: D must be a multiple of 128 up to 1152 (got %d)", D);
+    if (table_rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: table_rows must be >= 1 (got %d)", table_rows);
+    if (t == nullptr || w0 == nullptr || b0 == nullptr || w2 == nullptr || b2 == nullptr || table == nullptr || tf_out == nullptr ||
+        h1_out == nullptr || c_bf16 == nullptr)
+        return fail(nullptr, "lfm_dbg_dit_condition: only y may be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        return launch_dit_condition(ctx, static_cast<cudaStream_t>(stream), t, t_numel, y, rows, D, w0, b0, w2, b2, table, table_rows,
+                                    tf_out, h1_out, static_cast<__nv_bfloat16*>(c_bf16));
+    });
+}
+
+static bool dit_patch_ok(int p) { return p == 2 || p == 4 || p == 8; }
+
+extern "C" int lfm_dbg_patch_embed(const float* x, int x_rows, const float* Wt, const float* bias, const float* pos, float* tok, int D,
+                                   int G, int C, int p, int M, void* stream) {
+    if (!dit_patch_ok(p)) return fail(nullptr, "lfm_dbg_patch_embed: p must be 2, 4 or 8 (got %d)", p);
+    if (p == 2 ? C != 4 : (C < 1 || 8 * C * p * p * (int)sizeof(float) > 48 * 1024))
+        return fail(nullptr, "lfm_dbg_patch_embed: C must be 4 at p = 2, and 8 C p^2 floats must fit 48 KB (got C %d, p %d)", C, p);
+    if (D < 4 || D % 4 != 0) return fail(nullptr, "lfm_dbg_patch_embed: D must be a positive multiple of 4 (got %d)", D);
+    if (G < 1 || x_rows < 1 || M < 1)
+        return fail(nullptr, "lfm_dbg_patch_embed: G, x_rows and M must be >= 1 (got %d, %d, %d)", G, x_rows, M);
+    if (x == nullptr || Wt == nullptr || bias == nullptr || pos == nullptr || tok == nullptr)
+        return fail(nullptr, "lfm_dbg_patch_embed: x, Wt, bias, pos and tok must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        return launch_patch_embed(ctx, static_cast<cudaStream_t>(stream), x, x_rows, Wt, bias, pos, tok, D, G, C, p, M);
+    });
+}
+
+extern "C" int lfm_dbg_final_layer(const float* x, const float* shift, const float* scale, int mod_stride, const float* W, const float* bias,
+                                   float* v_net, int M, int D, int G, int C, int p, void* stream) {
+    if (!dit_patch_ok(p)) return fail(nullptr, "lfm_dbg_final_layer: p must be 2, 4 or 8 (got %d)", p);
+    if (p == 2 ? C != 4 : C < 1)
+        return fail(nullptr, "lfm_dbg_final_layer: C must be 4 at p = 2 (the kernel computes 16 outputs), >= 1 otherwise (got %d)", C);
+    if (D < 128 || D % 128 != 0 || D > 1536)
+        return fail(nullptr, "lfm_dbg_final_layer: D must be a multiple of 128 up to 1536 (got %d)", D);
+    if (mod_stride < 0 || mod_stride % 4 != 0)
+        return fail(nullptr, "lfm_dbg_final_layer: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
+    if (G < 1 || M < 1) return fail(nullptr, "lfm_dbg_final_layer: G and M must be >= 1 (got %d, %d)", G, M);
+    if (x == nullptr || shift == nullptr || scale == nullptr || W == nullptr || bias == nullptr || v_net == nullptr ||
+        !aligned16(shift) || !aligned16(scale))
+        return fail(nullptr, "lfm_dbg_final_layer: x, shift, scale, W, bias and v_net must not be NULL (shift and scale 16-byte aligned)");
+    return dbg_run([&](lfm_ctx* ctx) {
+        return launch_final_layer(ctx, static_cast<cudaStream_t>(stream), x, shift, scale, mod_stride, W, bias, v_net, M, D, G, C, p);
     });
 }
 

@@ -1,12 +1,15 @@
 """The GEMM epilogue stores whole 32-column groups with 16-byte accesses after a transpose within each quad of lanes, and
 falls back to the per-8-column stores for the N tail and for an output that is not 16-byte aligned.  Both paths must write
-the same bytes: the same product written to an aligned and to a misaligned (4 bytes off) output is compared bit for bit."""
+the same bytes: the same product written to an aligned and to a misaligned (4 bytes off) output is compared bit for bit, and both
+are held elementwise to the fp64 product (the bounds of tests/test_gpu_dit_kernels.py), so that a mistake both paths share is seen."""
 import ctypes as C
 
 import pytest
 import torch
 
 from lfm_b200 import _lib
+from tests import test_gpu_kernels as tk
+from tests.test_gpu_dit_kernels import gemm_expect, gemm_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -33,8 +36,8 @@ def test_vector_and_scalar_stores_agree(M, N, K, epi, bn):
         assert rc == 0, _lib.last_error()
         outs.append(buf[off:off + M * N].clone())
     assert torch.equal(outs[0], outs[1])
-    acc = a.double() @ w.double().t() + bias.double()
-    ref = {0: acc, 1: torch.nn.functional.gelu(acc, approximate="tanh"), 3: acc,
-           2: x0.double().view(M, N) + gate.double()[torch.arange(M, device="cuda") // 256] * acc}[epi]
+    acc, absacc = gemm_ref(a, w, bias)
+    ref, bound = gemm_expect(epi, acc, absacc, K, x0.view(M, N), gate[torch.arange(M, device="cuda") // 256])
     err = (outs[0].double().view(M, N) - ref).norm() / ref.norm()
     assert err < (4e-3 if epi < 2 else 1e-5)
+    tk.assert_within(outs[0].view(M, N), ref, bound, f"gemm {M}x{N}x{K} epi {epi} bn {bn}")

@@ -130,6 +130,46 @@ def test_kernel_entries_refuse_bad_arguments(lib):
     refused(mma(None, None, 1, 1, 64, 64, 72, None), "head_dim")
     refused(mma(None, None, 1, 1, 256, 128, 0, None), "T")
     refused(mma(None, None, 1, 1, 48, 64, 64, None), "T")
+    # lfm_dbg_gemm_reversed: lfm_dbg_gemm's checks, under its own name
+    rev = lib.lfm_dbg_gemm_reversed
+    refused(rev(None, None, None, None, None, 0, 1, 128, 128, 64, 3, 640, None), "block_n")
+    refused(rev(None, None, None, None, None, 0, 1, 128, 128, 96, 3, 0, None), "lfm_dbg_gemm_reversed: K")
+    refused(rev(None, None, None, None, None, 0, 1, 128, 128, 64, 4, 0, None), "epilogue")
+    # lfm_dbg_ln_modulate(x, y, shift, scale, mod_stride, rows_per_sample, M, D, down, stream)
+    ln = lib.lfm_dbg_ln_modulate
+    refused(ln(None, None, None, None, 0, 256, 512, 512, 0, None), "D")         # D / 128 = 4 has no instantiation
+    refused(ln(None, None, None, None, 0, 256, 512, 1000, 0, None), "D")
+    refused(ln(None, None, None, None, 0, 24, 512, 1024, 0, None), "rows_per_sample")
+    refused(ln(None, None, None, None, 0, 0, 512, 1024, 0, None), "rows_per_sample")
+    refused(ln(None, None, None, None, 0, 256, 0, 1024, 0, None), "M")
+    refused(ln(None, None, None, None, 6, 256, 512, 1024, 0, None), "mod_stride")
+    refused(ln(None, None, None, None, 0, 256, 512, 1024, 2, None), "down")
+    refused(ln(None, None, None, None, 0, 256, 512, 1024, 0, None), "NULL")
+    # lfm_dbg_dit_condition(t, t_numel, y, rows, D, w0, b0, w2, b2, table, table_rows, tf, h1, c, stream)
+    cond = lib.lfm_dbg_dit_condition
+    refused(cond(None, 1, None, 0, 384, None, None, None, None, None, 11, None, None, None, None), "rows")
+    refused(cond(None, 3, None, 4, 384, None, None, None, None, None, 11, None, None, None, None), "t_numel")
+    refused(cond(None, 1, None, 4, 1280, None, None, None, None, None, 11, None, None, None, None), "D")
+    refused(cond(None, 1, None, 4, 200, None, None, None, None, None, 11, None, None, None, None), "D")
+    refused(cond(None, 1, None, 4, 384, None, None, None, None, None, 0, None, None, None, None), "table_rows")
+    refused(cond(None, 4, None, 4, 384, None, None, None, None, None, 11, None, None, None, None), "NULL")
+    # lfm_dbg_patch_embed(x, x_rows, Wt, bias, pos, tok, D, G, C, p, M, stream)
+    pe = lib.lfm_dbg_patch_embed
+    refused(pe(None, 1, None, None, None, None, 384, 16, 4, 3, 256, None), "p")
+    refused(pe(None, 1, None, None, None, None, 384, 16, 3, 2, 256, None), "C")
+    refused(pe(None, 1, None, None, None, None, 384, 16, 32, 8, 256, None), "C")        # 8 x 2048 floats: 64 KB of shared memory
+    refused(pe(None, 1, None, None, None, None, 386, 16, 4, 2, 256, None), "D")
+    refused(pe(None, 0, None, None, None, None, 384, 16, 4, 2, 256, None), "x_rows")
+    refused(pe(None, 1, None, None, None, None, 384, 16, 4, 2, 256, None), "NULL")
+    # lfm_dbg_final_layer(x, shift, scale, mod_stride, W, bias, v_net, M, D, G, C, p, stream)
+    fl = lib.lfm_dbg_final_layer
+    refused(fl(None, None, None, 0, None, None, None, 256, 384, 16, 4, 6, None), "p")
+    refused(fl(None, None, None, 0, None, None, None, 256, 384, 16, 3, 2, None), "C")    # the p = 2 kernel computes 16 outputs
+    refused(fl(None, None, None, 0, None, None, None, 256, 1664, 16, 4, 2, None), "D")   # > 1536
+    refused(fl(None, None, None, 0, None, None, None, 256, 320, 16, 4, 4, None), "D")
+    refused(fl(None, None, None, 2, None, None, None, 256, 384, 16, 4, 2, None), "mod_stride")
+    refused(fl(None, None, None, 0, None, None, None, 0, 384, 16, 4, 2, None), "M")
+    refused(fl(None, None, None, 0, None, None, None, 256, 384, 16, 4, 2, None), "NULL")
 
 
 def _unet_desc(cfg):
