@@ -207,6 +207,13 @@ int lfm_dbg_gemm(const void* a_bf16, const void* w_bf16, const float* bias, void
  * every other GEMM); same arguments and results. */
 int lfm_dbg_gemm_reversed(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
                           int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream);
+/* lfm_dbg_gemm with the epilogue's store path chosen by the caller, so that the paths can be compared in one build.  reverse:
+ * as lfm_dbg_gemm_reversed when non-zero.  tma_store: -1 staged in shared memory and written by TMA stores whenever the output
+ * allows it (16-byte aligned base and pitch; what lfm_dbg_gemm and the network do), 0 register stores, 1 TMA stores (rejected
+ * when the output does not allow them).  Both paths write the same bits. */
+int lfm_dbg_gemm_path(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                      int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, int reverse,
+                      int tma_store, void* stream);
 /* The DiT's LayerNorm (no affine, eps 1e-6) + adaLN modulate: y[r] = bf16((x[r] - mean) rstd (1 + scale[b]) + shift[b]),
  * b = r / rows_per_sample, the vectors of sample b at shift / scale + b * mod_stride (0: one shared row).  x fp32 [M, D],
  * y bf16 [M, D].  D = 128 x {2, 3, 6, 8, 9}; rows_per_sample a multiple of 16; down 1 sweeps the rows downwards.  All pointers

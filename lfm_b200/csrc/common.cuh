@@ -63,6 +63,19 @@ LFM_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// named barriers and stmatrix
+
+// bar.sync on barrier `id` (1 .. 15; 0 is __syncthreads) among `threads` threads.
+LFM_DEVICE void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
+// Four 8 x 8 bf16 matrices from the mma fragment layout (lane l holds row l / 4, columns 2 (l % 4), + 1 of each, in r0 .. r3)
+// to shared memory: lane l gives the address of row l % 8 of matrix l / 8 (16 contiguous bytes).
+LFM_DEVICE void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+
+// ------------------------------------------------------------------------------------------------
 // TMA
 
 LFM_DEVICE void prefetch_tmap(const CUtensorMap* m) {

@@ -5,7 +5,9 @@
 // One 128 x BN output tile per CTA and step of a persistent tile loop (BN = 128 or 256).  Both operands are K-major,
 // staged by TMA into 128B-swizzled shared memory (64-element K slabs) in a ring of kStages slots.
 // Warp groups (384 threads): group 0 = TMA producer (one thread), groups 1 and 2 = consumers: each multiplies its 64 rows
-// of the tile with wgmma.m64nBNk16 into registers (fp32) and applies the fused epilogue straight from those registers.
+// of the tile with wgmma.m64nBNk16 into registers (fp32) and applies the fused epilogue to them.  Given an output tensor map
+// (GemmEpi::out_map) the epilogue stages 64-row sub-tiles in shared memory and writes each with one TMA store
+// (epilogue_tma); otherwise it stores straight from the registers.
 //
 // Fused epilogues (reference ops they replace):
 //   EPI_BIAS_BF16       out = bf16(acc + bias)                       attn.qkv       (timm Attention)
@@ -43,6 +45,11 @@ struct GemmEpi {
     // Walk the M blocks from the last to the first.  Consecutive kernels of a network alternate direction so that
     // each one starts on the rows its producer touched LAST - the part still resident in L2.
     int reverse_m = 0;
+    // Tensor map of `out` (make_tmap_out: 64-row boxes of 128 bytes, 128-byte swizzle), or nullptr.  Given, the epilogue stages
+    // each 64-row sub-tile in shared memory and writes it with one TMA store (the residual stream is TMA-loaded into the same
+    // buffer first).  The launch passes the map itself as a kernel parameter; the kernel only tests this pointer.  Plain
+    // GEMMs without GroupNorm statistics only; sub-tiles with rows past M keep the register stores.
+    const CUtensorMap* out_map = nullptr;
 };
 constexpr int kGnBinReplicas = 16;
 constexpr double kGnFixScale = 268435456.0;  // 2^28: the sum
@@ -72,14 +79,18 @@ constexpr int kGemmBlockM = 128;
 constexpr int kGemmBlockK = 64;  // 64 bf16 = one 128-byte swizzle row
 constexpr int kGemmThreads = 384;
 constexpr int kGemmBoxRows = 128;  // rows of the TMA box of both operand tensor maps
+constexpr int kGemmOutRows = 64;   // rows of an output sub-tile (one consumer warp group) and of the output tensor map's box
+constexpr int kGemmOutBytes = kGemmOutRows * 128;  // one staging buffer: 64 rows of 128 bytes (64 bf16 / 32 fp32 columns)
 
 template <int BN>
 struct GemmCfg {
     static constexpr int kABytes = kGemmBlockM * kGemmBlockK * 2;
     static constexpr int kBBytes = BN * kGemmBlockK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kStages = (BN == 256) ? 4 : 6;  // 192 KB of the 227 KB a block may have
-    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int kStages = (BN == 256) ? 4 : 6;  // 192 KB of operand slabs
+    static constexpr int kOutBytes = 2 * 2 * kGemmOutBytes;  // two staging buffers per consumer warp group: 32 KB
+    static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(kSmemBytes <= 227 * 1024, "more shared memory than an sm_90 block may have");
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -281,6 +292,111 @@ LFM_DEVICE void epilogue_store_32(const float* acc, const GemmEpi& ep, int c32, 
     }
 }
 
+// Epilogue of one consumer warp group's 64 rows (grow .. grow + 63, all < M) through shared memory: the BN columns go out in
+// sub-tiles of 128 bytes per row (64 bf16 / 32 fp32 columns), each staged in one of the group's two buffers `sc` in the
+// output map's 128-byte swizzle (16-byte chunk c of row r at chunk c ^ (r % 8)) and written by one TMA store, which drains
+// while the group fills the other buffer.  The residual stream's sub-tile is TMA-loaded into its buffer one sub-tile ahead
+// (the first one before the main loop), updated in place and stored back.  Per element the arithmetic is the register path's.
+// `obuf` (the buffer of the next sub-tile) and `xphase` (parity bit per buffer of the load barriers `xb`) carry over tiles.
+template <int BN, int EPI>
+LFM_DEVICE void epilogue_tma(const float* acc, const GemmEpi& ep, const CUtensorMap* tmap_c, uint8_t* sc, uint64_t* xb, int& obuf,
+                             uint32_t& xphase, int grow, int nbase, int N, int bar_id) {
+    constexpr bool kBf16 = EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16;
+    constexpr int kCols = kBf16 ? 64 : 32;
+    const int lane = threadIdx.x & 31, q = lane & 3, warp_in = (threadIdx.x >> 5) & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int r0 = warp_in * 16 + (lane >> 2);  // this lane's rows r0, r0 + 8 of the sub-tile; both are (lane / 4) mod 8
+    const float* gate0 = nullptr;
+    const float* gate1 = nullptr;
+    if (EPI == EPI_GATE_RESID_F32 && ep.gate != nullptr) {
+        gate0 = ep.gate + static_cast<size_t>((grow + r0) / ep.rows_per_sample) * ep.gate_stride;
+        gate1 = ep.gate + static_cast<size_t>((grow + r0 + 8) / ep.rows_per_sample) * ep.gate_stride;
+    }
+#pragma unroll
+    for (int s = 0; s < BN / kCols; ++s) {
+        const int c0 = nbase + s * kCols;  // warp-uniform
+        if (c0 >= N) break;
+        uint8_t* buf = sc + obuf * kGemmOutBytes;
+        if (EPI == EPI_GATE_RESID_F32) {
+            if (leader) {
+                tma_store_wait_read<0>();  // the other buffer's store (the previous sub-tile) has read it
+                if (s + 1 < BN / kCols && c0 + kCols < N) {
+                    mbar_arrive_expect_tx(&xb[obuf ^ 1], kGemmOutBytes);
+                    tma_load_2d(sc + (obuf ^ 1) * kGemmOutBytes, tmap_c, &xb[obuf ^ 1], c0 + kCols, grow);
+                }
+            }
+            mbar_wait(&xb[obuf], (xphase >> obuf) & 1u);
+            xphase ^= 1u << obuf;
+        } else {
+            if (leader) tma_store_wait_read<1>();  // the store issued from this buffer two sub-tiles ago has read it
+            named_bar_sync(bar_id, 128);
+        }
+        const uint32_t base = smem_u32(buf);
+        if constexpr (kBf16) {
+#pragma unroll
+            for (int p = 0; p < 4; ++p) {
+                uint32_t rr[4];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int i = s * 8 + 2 * p + h;
+                    const int col = nbase + 8 * i + 2 * q;
+                    float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
+                    if (ep.bias != nullptr && col < N) {
+                        const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
+                        v0 += b0, v1 += b1, v2 += b0, v3 += b1;
+                    }
+                    if (EPI == EPI_BIAS_GELU_BF16) {
+                        v0 = gelu_tanh(v0), v1 = gelu_tanh(v1), v2 = gelu_tanh(v2), v3 = gelu_tanh(v3);
+                    }
+                    rr[2 * h] = pack_bf16x2(v0, v1);
+                    rr[2 * h + 1] = pack_bf16x2(v2, v3);
+                }
+                // matrix m = lane / 8: rows + 8 (m & 1), chunk 2 p + m / 2
+                const int m = lane >> 3, row = warp_in * 16 + (m & 1) * 8 + (lane & 7), chunk = 2 * p + (m >> 1);
+                stmatrix_x4(base + row * 128 + ((chunk ^ (lane & 7)) << 4), rr[0], rr[1], rr[2], rr[3]);
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = s * 4 + j;
+                const int col = nbase + 8 * i + 2 * q;
+                if (col >= N) continue;  // past the tail: the TMA store clips these columns
+                float v0 = acc[4 * i], v1 = acc[4 * i + 1], v2 = acc[4 * i + 2], v3 = acc[4 * i + 3];
+                if (ep.bias != nullptr) {
+                    const float b0 = __ldg(ep.bias + col), b1 = __ldg(ep.bias + col + 1);
+                    v0 += b0, v1 += b1, v2 += b0, v3 += b1;
+                }
+                const int off = (((2 * j + (q >> 1)) ^ ((lane >> 2) & 7)) << 4) + 8 * (q & 1);
+                float2* p0 = reinterpret_cast<float2*>(buf + r0 * 128 + off);
+                float2* p1 = reinterpret_cast<float2*>(buf + (r0 + 8) * 128 + off);
+                if (EPI == EPI_BIAS_F32) {
+                    *p0 = make_float2(v0, v1);
+                    *p1 = make_float2(v2, v3);
+                } else {
+                    float2 x = *p0, y = *p1;
+                    if (gate0 != nullptr) {
+                        x.x = fmaf(__ldg(gate0 + col), v0, x.x);
+                        x.y = fmaf(__ldg(gate0 + col + 1), v1, x.y);
+                        y.x = fmaf(__ldg(gate1 + col), v2, y.x);
+                        y.y = fmaf(__ldg(gate1 + col + 1), v3, y.y);
+                    } else {
+                        x.x += v0, x.y += v1, y.x += v2, y.y += v3;
+                    }
+                    *p0 = x;
+                    *p1 = y;
+                }
+            }
+        }
+        fence_proxy_async();  // the generic-proxy writes above, before the TMA store reads them
+        named_bar_sync(bar_id, 128);
+        if (leader) {
+            tma_store_2d(tmap_c, buf, c0, grow);
+            tma_store_commit();
+        }
+        obuf ^= 1;
+    }
+}
+
 // Work items: (tile, k-slice).  ksplit > 1 (split-K, for GEMMs with far fewer tiles than SMs): every slice stores its fp32
 // partial tile, without bias, into its own slab of ep.out (row offset slice * split_row_pitch); a separate kernel adds the
 // slabs in a fixed order.
@@ -288,6 +404,7 @@ template <int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the 4-D NHWC activation of a convolution), box 128 rows
                 const __grid_constant__ CUtensorMap tmap_b,  // W [N, K], box {64, 128}
+                const __grid_constant__ CUtensorMap tmap_c,  // out, when ep.out_map != nullptr (make_tmap_out)
                 int M, int N, int K, GemmEpi ep, ConvGeom cg, int ksplit, int split_row_pitch) {
     using Cfg = GemmCfg<BN>;
     constexpr int kStages = Cfg::kStages;
@@ -295,9 +412,11 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
-    uint64_t* full_bar = bars;             // [kStages] TMA -> consumers
-    uint64_t* empty_bar = bars + kStages;  // [kStages] consumers (8 warps) -> TMA
+    uint8_t* smem_c = smem + kStages * Cfg::kStageBytes;  // [consumer group][2] staging buffers of the TMA-store epilogue
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + Cfg::kOutBytes);
+    uint64_t* full_bar = bars;                 // [kStages] TMA -> consumers
+    uint64_t* empty_bar = bars + kStages;      // [kStages] consumers (8 warps) -> TMA
+    uint64_t* x_bar = bars + 2 * kStages;      // [consumer group][2] residual-stream sub-tile loaded into a staging buffer
 
     const int wg = threadIdx.x >> 7;
     const int lane = threadIdx.x & 31;
@@ -318,10 +437,12 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmap_a);
         prefetch_tmap(&tmap_b);
+        if (ep.out_map != nullptr) prefetch_tmap(&tmap_c);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 8);
         }
+        for (int s = 0; s < 4; ++s) mbar_init(&x_bar[s], 1);
         fence_barrier_init();
         fence_proxy_async();
     }
@@ -386,10 +507,22 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
         float acc[BN / 2];
         int stage = 0;
         uint32_t phase = 0;
+        uint8_t* sc = smem_c + cw * 2 * kGemmOutBytes;
+        uint64_t* xb = x_bar + 2 * cw;
+        int obuf = 0;
+        uint32_t xphase = 0;
+        const bool leader = (threadIdx.x & 127) == 0;
         for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
             int m_blk, n_blk, ks;
             decode(item, m_blk, n_blk, ks);
             const int kb0 = ks * kb_per, kb1 = min(num_kb, kb0 + kb_per);
+            const int grow = m_blk * kGemmBlockM + cw * 64;  // first row of this warp group
+            const bool tma_epi = ep.out_map != nullptr && grow + kGemmOutRows <= M;  // warp-group-uniform
+            if (EPI == EPI_GATE_RESID_F32 && tma_epi && leader) {  // the first residual sub-tile loads under the main loop
+                tma_store_wait_read<0>();
+                mbar_arrive_expect_tx(&xb[obuf], kGemmOutBytes);
+                tma_load_2d(sc + obuf * kGemmOutBytes, &tmap_c, &xb[obuf], n_blk * BN, grow);
+            }
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
             int prev_stage = 0;
@@ -417,6 +550,10 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
             if (kb1 > kb0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            if (tma_epi) {
+                epilogue_tma<BN, EPI>(acc, ep, &tmap_c, sc, xb, obuf, xphase, grow, n_blk * BN, N, 1 + cw);
+                continue;
+            }
 
             // ---- epilogue from registers.  wgmma accumulator layout: acc[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1};
             // acc[4 i + {2, 3}] = row r0 + 8, same columns; r0 = 16 warp + lane / 4 within the warp group's 64 rows.
@@ -520,6 +657,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 }
             }
         }
+        if (leader) tma_store_wait<0>();  // the stores are complete (not only read) before the grid can count as finished
     }
 }
 

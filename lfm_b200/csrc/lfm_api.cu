@@ -74,6 +74,22 @@ static bool make_tmap_bf16_ld(CUtensorMap* m, const void* base, uint64_t rows, u
 static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     return make_tmap_bf16_ld(m, base, rows, cols, cols, box_rows);
 }
+// GEMM output [rows, cols] (bf16, or fp32 when f32) with a row pitch of ld elements, for the TMA-store epilogue (GemmEpi::out_map):
+// box = 128 bytes x kGemmOutRows rows in the 128-byte swizzle of the staging buffers.  False when the map cannot exist (base or
+// pitch not a multiple of 16 bytes): such outputs keep the register stores.
+static bool make_tmap_out(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, bool f32) {
+    const uint64_t es = f32 ? 4 : 2;
+    EncodeTiledFn fn = get_encode_fn();
+    if (fn == nullptr || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * es) % 16 != 0) return false;
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {ld * es};
+    cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / es), static_cast<cuuint32_t>(kGemmOutRows)};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims,
+                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
 
 // ------------------------------------------------------------------------------------------------
 // kernel launch helpers
@@ -130,7 +146,8 @@ static cudaError_t launch_gemm_inst(cudaStream_t s, const CUtensorMap& ta, const
     if (cudaError_t e = smem_opt_in(once, kern, GemmCfg<BN>::kSmemBytes)) return e;
     const int items = ((M + kGemmBlockM - 1) / kGemmBlockM) * ((N + BN - 1) / BN) * ksplit;
     const int grid = items < g_num_sms ? items : g_num_sms;
-    return launch_k(kern, dim3(grid), kGemmThreads, GemmCfg<BN>::kSmemBytes, s, ta, tb, M, N, K, ep, cg, ksplit, split_row_pitch);
+    const CUtensorMap& tc = ep.out_map != nullptr ? *ep.out_map : ta;  // unread without an out_map
+    return launch_k(kern, dim3(grid), kGemmThreads, GemmCfg<BN>::kSmemBytes, s, ta, tb, tc, M, N, K, ep, cg, ksplit, split_row_pitch);
 }
 
 // softmax(q k^T / 8) v for 256 tokens, head_dim 64, timm qkv order (attention_wgmma.cuh); tqkv: box {64, kGemmBoxRows} over [rows, 3 C]
@@ -152,12 +169,15 @@ static int pick_block_n(int M, int N) {
 
 // A and W are tensor maps with a box of {64, kGemmBoxRows} (make_tmap_bf16 / make_tmap_act4d); block_n = 128 or 256
 // (0: pick_block_n).  The batched GEMMs of ConvGeom need block_n 256 when N is a multiple of 256 (W rows of one group).
+// Only plain 2-D GEMMs (no taps, no batching, no split-K) without GroupNorm statistics store through ep.out_map.
 static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int epi,
                                int block_n, const GemmEpi& ep, const ConvGeom& cg = ConvGeom{0, 0, 0, 0, 1}, int ksplit = 1,
                                int split_row_pitch = 0) {
     if (block_n == 0) block_n = cg.batch_m > 0 ? 256 : pick_block_n(M, N);
+    GemmEpi e = ep;
+    if (cg.taps != 0 || cg.batch_m != 0 || ksplit != 1 || ep.gn_bins != nullptr) e.out_map = nullptr;
 #define LFM_GEMM_CASE(BN, E) \
-    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E>(s, ta, tb, M, N, K, ep, cg, ksplit, split_row_pitch);
+    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E>(s, ta, tb, M, N, K, e, cg, ksplit, split_row_pitch);
     LFM_GEMM_CASE(256, EPI_BIAS_BF16)
     LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
     LFM_GEMM_CASE(256, EPI_GATE_RESID_F32)
@@ -265,6 +285,7 @@ struct lfm_ctx {
     float *x_tok = nullptr, *mod = nullptr, *tfreq = nullptr, *h1 = nullptr, *v_net = nullptr;
     __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
     CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
+    CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok, tmo_mod;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
     CUtensorMap tm_qkv_attn;  // qkv as read by the 256-token attention (timm order only)
 
     // solver state
@@ -619,6 +640,10 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, kGemmBoxRows);
     if (!ctx->qkv_head_major) ok &= make_tmap_bf16(&ctx->tm_qkv_attn, ctx->qkv, M, 3 * Dq, kGemmBoxRows);
+    ok &= make_tmap_out(&ctx->tmo_qkv, ctx->qkv, M, 3 * Dq, 3 * Dq, false);
+    ok &= make_tmap_out(&ctx->tmo_hmid, ctx->hmid, M, Hd, Hd, false);
+    ok &= make_tmap_out(&ctx->tmo_x_tok, ctx->x_tok, M, D, D, true);
+    ok &= make_tmap_out(&ctx->tmo_mod, ctx->mod, R, ctx->Nmod, ctx->Nmod, true);
     for (auto& b : ctx->blk) {
         ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, kGemmBoxRows);
         ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, kGemmBoxRows);
@@ -712,6 +737,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         return 1;
     {   // all adaLN modulation vectors of the network in one GEMM: mod[crows, (6L+2) D]
         GemmEpi ep{ctx->b_mod, ctx->mod, ctx->Nmod, nullptr, 0, 1};
+        ep.out_map = &ctx->tmo_mod;
         COUNT_LAUNCH(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
     }
     const int ps = ctx->d.patch_size;
@@ -731,6 +757,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
             ep.reverse_m = next_dir();
+            ep.out_map = &ctx->tmo_qkv;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, 0, ep));
         }
         {
@@ -747,17 +774,20 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         {
             GemmEpi ep{b.b_proj, ctx->x_tok, D, mb + 2 * D, Nmod, T};  // x += gate_msa * proj(...)   (models/DiT.py:129)
             ep.reverse_m = next_dir();
+            ep.out_map = &ctx->tmo_x_tok;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
         }
         COUNT_LAUNCH(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, next_dir()));
         {
             GemmEpi ep{b.b_fc1, ctx->hmid, Hd, nullptr, 0, T};
             ep.reverse_m = next_dir();
+            ep.out_map = &ctx->tmo_hmid;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, 0, ep));
         }
         {
             GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};  // x += gate_mlp * fc2(...)   (models/DiT.py:130)
             ep.reverse_m = next_dir();
+            ep.out_map = &ctx->tmo_x_tok;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
         }
     }
@@ -1338,18 +1368,25 @@ static int dbg_run(Op&& op) {
 }
 
 // lfm_dbg_gemm and lfm_dbg_gemm_reversed: `reverse` sets GemmEpi::reverse_m, as the network does on every other GEMM.
+// lfm_dbg_gemm_path: tma_store = 0 / 1 forces the epilogue's stores.  By default (-1) the output is stored through a tensor map
+// whenever one can be made for it (16-byte aligned base and pitch), as in the network.
 static int dbg_gemm(const char* who, int reverse, const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
-                    int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream) {
+                    int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream,
+                    int tma_store = -1) {
     if (K % 64 != 0 || N % 8 != 0) return fail(nullptr, "%s: K must be a multiple of 64 and N of 8", who);
     if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(nullptr, "%s: unknown epilogue %d", who, epi);
     if (block_n != 0 && block_n != 128 && block_n != 256)
         return fail(nullptr, "%s: block_n must be 0, 128 or 256 (got %d)", who, block_n);
+    if (tma_store < -1 || tma_store > 1) return fail(nullptr, "%s: tma_store must be -1, 0 or 1 (got %d)", who, tma_store);
     return dbg_run([&](lfm_ctx* ctx) {
-        CUtensorMap ta, tb;
+        CUtensorMap ta, tb, tc;
         if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
             return fail(ctx, "%s: tensor map encode failed", who);
+        const bool has_c = tma_store != 0 && make_tmap_out(&tc, out, M, N, N, epi >= EPI_GATE_RESID_F32);
+        if (tma_store == 1 && !has_c) return fail(ctx, "%s: no output tensor map for this output (16-byte alignment)", who);
         GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
         ep.reverse_m = reverse;
+        ep.out_map = has_c ? &tc : nullptr;
         CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
         return 0;
     });
@@ -1366,6 +1403,13 @@ extern "C" int lfm_dbg_gemm_reversed(const void* a_bf16, const void* w_bf16, con
                                      void* stream) {
     return dbg_gemm("lfm_dbg_gemm_reversed", 1, a_bf16, w_bf16, bias, out, gate, gate_stride, rows_per_sample, M, N, K, epi, block_n,
                     stream);
+}
+
+extern "C" int lfm_dbg_gemm_path(const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
+                                 int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, int reverse,
+                                 int tma_store, void* stream) {
+    return dbg_gemm("lfm_dbg_gemm_path", reverse != 0, a_bf16, w_bf16, bias, out, gate, gate_stride, rows_per_sample, M, N, K, epi,
+                    block_n, stream, tma_store);
 }
 
 // The DiT's own kernels, each through the helper launch_network calls.
