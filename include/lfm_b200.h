@@ -143,6 +143,21 @@ int lfm_create_vae(const lfm_vae_desc* desc, int device, lfm_ctx** out);
  *   out_u8:  [B, 8s, 8s, 3] uint8 = (clamp((sample + 1) / 2, 0, 1) * 255).permute(0, 2, 3, 1).to(uint8), or NULL */
 int lfm_decode(lfm_ctx* ctx, const float* z, int B, float* out_f32, uint8_t* out_u8, void* stream);
 
+/* AutoencoderKL(...).encode (downstream_tasks/test_flow_latent_inpainting.py:147): a context for the ENCODER, described by the
+ * same struct, with out_channels read as the image channels (3) and latent_size = image side / 8 (16, 32 or 64).  lfm_set_param
+ * takes the `encoder.*` and `quant_conv.*` entries of the diffusers state dict (attention projections under to_q / to_k / to_v /
+ * to_out.0); a decoder key is refused, as an encoder key is by an lfm_create_vae context.  lfm_finalize(max_batch) sizes the
+ * workspace for max_batch images per call. */
+int lfm_create_vae_encoder(const lfm_vae_desc* desc, int device, lfm_ctx** out);
+
+/* first_stage_model.encode(x).latent_dist's moments: quant_conv(encoder(x)).chunk(2) with the log-variance clamped to
+ * [-30, 20], as DiagonalGaussianDistribution stores them.  The caller draws the sample (mean + exp(0.5 logvar) * eps).
+ *   x:      [B, 3, S, S] fp32 NCHW (device), S = 8 latent_size
+ *   mean:   [B, 4, S / 8, S / 8] fp32 NCHW
+ *   logvar: [B, 4, S / 8, S / 8] fp32 NCHW
+ * An lfm_create_vae context refuses this call; an lfm_create_vae_encoder context refuses lfm_decode. */
+int lfm_encode(lfm_ctx* ctx, const float* x, int B, float* mean, float* logvar, void* stream);
+
 /* nn.Module.load_state_dict (test_flow_latent.py:142): one call per state-dict entry, `key` exactly as in the
  * reference state_dict (SURVEY.md 8(b)); `ptr` may be a host or a device pointer (fp32).  The data is copied
  * (GEMM weights are repacked to bf16).  Unknown key or wrong shape -> error (strict=True behaviour). */
@@ -262,12 +277,23 @@ int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void
  * lfm_dbg_conv.  Arguments are checked before the device is touched. */
 int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
                       int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
+/* The VAE encoder's Downsample2D(padding=0), F.pad(x, (0, 1, 0, 1)) then a 3x3 stride-2 convolution, as the network runs it: the
+ * extra bottom row and right column are the tensor map's zero fill.  side 8..512 (a power of 2; output rows wider than 128 pixels
+ * run on 128-pixel row segments), stride 2; every other argument as lfm_dbg_conv.  Arguments are checked before the device is
+ * touched. */
+int lfm_dbg_conv_down(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B, int side,
+                      int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream);
 /* The UNet programs' conv_in (3x3, pad 1, fp32) as the network runs it: input channels [a | b] of two NCHW fp32 sources, a with a_ch
  * channels and image i at a + i * a_stride, b likewise (NULL when b_ch = 0); a_ch + b_ch in [3, 16].  w fp32 [Cout, a_ch + b_ch, 3, 3],
- * bias fp32 [Cout], out fp32 NHWC [B, side, side, Cout].  side in [1, 256] (with (a_ch + b_ch) * 3 * (side + 4) floats in 48 KB).
+ * bias fp32 [Cout], out fp32 NHWC [B, side, side, Cout].  side in [1, 256], or 512 with 3 channels (the VAE encoder's image input),
+ * with (a_ch + b_ch) * 3 * (side + 4) floats in 48 KB.
  * Arguments are checked before the device is touched. */
 int lfm_dbg_conv_in(const float* a, int a_ch, long long a_stride, const float* b, int b_ch, long long b_stride, const float* w,
                     const float* bias, float* out, int B, int side, int Cout, void* stream);
+/* The VAE encoder's tail as lfm_encode runs it: in = conv_out's output, NHWC fp32 [B * HW, 8] (16-byte aligned); w fp32 [8, 8]
+ * (quant_conv.weight), bias fp32 [8]; mean = quant_conv channels 0..3 and logvar = clamp(channels 4..7, -30, 20), NCHW fp32
+ * [B, 4, HW].  Arguments are checked before the device is touched. */
+int lfm_dbg_vae_quant(const float* in, const float* w, const float* bias, float* mean, float* logvar, int B, int HW, void* stream);
 /* The batched GEMM of the VAE mid-block attention: M = B * out_hw rows in groups of batch_m; group g computes
  * out[g rows] = A[rows] W[g * b_batch_rows .. + N]^T (+ bias), A row = row % a_mod when a_mod > 0 (A shared by all groups).
  * a: bf16 [a_rows, K] with row pitch a_ld, w: bf16 [w_rows, K] with row pitch w_ld (column windows of wider matrices);

@@ -46,6 +46,8 @@ SYMBOLS = {
     "lfm_create_edm": (C.c_int, [C.POINTER(EdmDesc), C.c_int, C.POINTER(_P)]),
     "lfm_create_vae": (C.c_int, [C.POINTER(VaeDesc), C.c_int, C.POINTER(_P)]),
     "lfm_decode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "lfm_create_vae_encoder": (C.c_int, [C.POINTER(VaeDesc), C.c_int, C.POINTER(_P)]),
+    "lfm_encode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "lfm_set_param": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.POINTER(C.c_int64), C.c_int]),
     "lfm_finalize": (C.c_int, [_P, C.c_int]),
     "lfm_set_condition": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
@@ -71,7 +73,9 @@ SYMBOLS = {
     "lfm_dbg_attention_mma": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv_wide": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_conv_down": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv_in": (C.c_int, [_P, C.c_int, C.c_longlong, _P, C.c_int, C.c_longlong, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_vae_quant": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P]),
     "lfm_dbg_gemm_batched": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int,
                                        C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_groupnorm": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P,

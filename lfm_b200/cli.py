@@ -106,7 +106,9 @@ def build_parser():
     return p
 
 
-def load_model(args, device):
+def load_model(args, device, ckpt_path=None):
+    """create_network(args) with --synthetic_init weights, or the checkpoint at `ckpt_path` (default: the generation
+    script's ./saved_info/latent_flow/... path) with its "module." prefix stripped."""
     from . import DhariwalUNet, UNetModel, create_network
     from .synthetic import synthetic_edm_state_dict, synthetic_state_dict, synthetic_unet_state_dict
     with torch.device("meta"):
@@ -116,7 +118,7 @@ def load_model(args, device):
                 else synthetic_edm_state_dict if isinstance(model, DhariwalUNet) else synthetic_state_dict)
         sd = make(model, args.synthetic_init)
     else:
-        path = "./saved_info/latent_flow/{}/{}/model_{}.pth".format(args.dataset, args.exp, args.epoch_id)
+        path = ckpt_path or "./saved_info/latent_flow/{}/{}/model_{}.pth".format(args.dataset, args.exp, args.epoch_id)
         ckpt = torch.load(path, map_location="cpu")
         for key in list(ckpt.keys()):            # test_flow_latent.py:140-141 (strip "module.")
             ckpt[key[7:]] = ckpt.pop(key)
@@ -143,8 +145,9 @@ def real_stats_path(args):
     return args.real_img_dir
 
 
-def load_vae(args, device):
-    """test_flow_latent.py:131 ``AutoencoderKL.from_pretrained(args.pretrained_autoencoder_ckpt).to(device)``."""
+def load_vae(args, device, with_encoder=False):
+    """test_flow_latent.py:131 ``AutoencoderKL.from_pretrained(args.pretrained_autoencoder_ckpt).to(device)``; the
+    native module holds the encoder too with `with_encoder`."""
     if args.no_decode:
         return None
     if args.vae == "diffusers":
@@ -155,11 +158,11 @@ def load_vae(args, device):
         return TorchVAE.from_pretrained(args.pretrained_autoencoder_ckpt).to(device)
     from .vae import AutoencoderKL, synthetic_vae_state_dict
     if args.synthetic_vae is not None:
-        vae = AutoencoderKL()
+        vae = AutoencoderKL(with_encoder=with_encoder)
         vae.load_state_dict(synthetic_vae_state_dict(vae, args.synthetic_vae), strict=True)
         return vae.to(device).eval()
     if os.path.isdir(args.pretrained_autoencoder_ckpt):
-        return AutoencoderKL.from_pretrained(args.pretrained_autoencoder_ckpt).to(device)
+        return AutoencoderKL.from_pretrained(args.pretrained_autoencoder_ckpt, with_encoder=with_encoder).to(device)
     print(f"'{args.pretrained_autoencoder_ckpt}' is not a local diffusers directory (no hub access here) and no "
           "--synthetic_vae seed was given: skipping the VAE decode, saving latents instead (--no_decode)")
     args.no_decode = True

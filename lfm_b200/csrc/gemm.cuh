@@ -61,8 +61,11 @@ constexpr double kGnFixScaleSq = 1048576.0;  // 2^20: the sum of squares
 // stages, W = 256 or 512; make_tmap_act4d refuses any other W above 128), so the matching input window of tap (r, s) is ONE
 // 4-D box.  A segment's box starts at w0 - 1 and ends at w0 + 128: the columns left of 0 and right of W - 1 are the TMA's
 // zero fill (the padding), the ones across an inner seam are the neighbouring segment's pixels.
+// Tap (r, s) of output pixel (h, w) reads input (stride * h + r - pad, stride * w + s - pad).  pad 1 is the symmetric padding of
+// every 3x3 convolution but one; pad 0 is diffusers' Downsample2D(padding=0), F.pad(x, (0, 1, 0, 1)) then a stride-2 conv: its
+// extra bottom row and right column are the out-of-bounds fill, so no padded copy of the input exists.
 struct ConvGeom {
-    int taps;     // 0 (GEMM), 9 (3x3, pad 1)
+    int taps;     // 0 (GEMM), 9 (3x3)
     int cblocks;  // C_in / 64
     int W;        // OUTPUT width
     int HW;       // OUTPUT height * width
@@ -73,6 +76,7 @@ struct ConvGeom {
     int batch_m = 0;
     int a_mod = 0;
     int b_batch_rows = 0;
+    int pad = 1;  // tap origin of a convolution (taps == 9): 1 or 0
 };
 
 constexpr int kGemmBlockM = 128;
@@ -482,7 +486,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                         tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kGemmBlockK, row_a);
                     } else {
                         const int r = tap / 3, sx = tap - 3 * r;
-                        tma_load_4d(sa, &tmap_a, &full_bar[stage], cb * 64, cg.stride * w0 + sx - 1, cg.stride * h0 + r - 1, img0);
+                        tma_load_4d(sa, &tmap_a, &full_bar[stage], cb * 64, cg.stride * w0 + sx - cg.pad, cg.stride * h0 + r - cg.pad, img0);
                         if (++cb == cg.cblocks) {
                             cb = 0;
                             ++tap;

@@ -243,8 +243,9 @@ struct ParamSlot {
     bool set = false;
 };
 
-// The network a context runs: lfm_create's DiT, or one of the three flavours of the UNet program (unet_host.inc, ctx->un).
-enum class NetKind { DIT, ADM, EDM, VAE };
+// The network a context runs: lfm_create's DiT, or one of the flavours of the UNet program (unet_host.inc, ctx->un): the two
+// UNets, the VAE decoder (lfm_create_vae) and the VAE encoder (lfm_create_vae_encoder).
+enum class NetKind { DIT, ADM, EDM, VAE, VAE_ENC };
 
 struct BlockW {
     __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;
@@ -826,7 +827,8 @@ static int check_ready(lfm_ctx* ctx, int rows, const char* who) {
 // check_ready for the entries that evaluate the velocity network (lfm_forward, lfm_sample_*), which a VAE context has not.
 static int check_velocity_ready(lfm_ctx* ctx, int rows, const char* who) {
     if (check_ready(ctx, rows, who)) return 1;
-    if (ctx->net == NetKind::VAE) return fail(ctx, "%s: a VAE context (lfm_create_vae) has no velocity network", who);
+    if (ctx->net == NetKind::VAE || ctx->net == NetKind::VAE_ENC)
+        return fail(ctx, "%s: a VAE context (lfm_create_vae / lfm_create_vae_encoder) has no velocity network", who);
     return 0;
 }
 
@@ -1537,13 +1539,22 @@ extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B
 
 static bool conv_out_side_ok(int s) { return s == 4 || s == 8 || s == 16 || s == 32 || s == 64 || s == 128 || s == 256; }
 
-// lfm_dbg_conv and lfm_dbg_conv_wide: the argument checks, then the launch.  `wide` selects the geometry and split-K rule of
-// lfm_dbg_conv_wide (output side 256 or 512, stride 1, never split along K) instead of lfm_dbg_conv's (output side 4..256,
-// stride 1 or 2, ksplit -1 = push_conv's plan, 1 = none, or 2..8).
-static int dbg_conv(const char* who, bool wide, const void* x_bf16, const void* w_bf16, const float* bias, void* out,
+// lfm_dbg_conv, lfm_dbg_conv_wide and lfm_dbg_conv_down: the argument checks, then the launch.  The mode selects the geometry
+// and split-K rule: CONV, lfm_dbg_conv's (output side 4..256, stride 1 or 2, tap origin 1, ksplit -1 = push_conv's plan, 1 = none,
+// or 2..8); WIDE, lfm_dbg_conv_wide's (output side 256 or 512, stride 1, never split along K); DOWN, lfm_dbg_conv_down's (the VAE
+// encoder's Downsample2D: stride 2 with tap origin 0, output side 4..256, split-K as CONV).
+enum class DbgConv { CONV, WIDE, DOWN };
+static int dbg_conv(const char* who, DbgConv mode, const void* x_bf16, const void* w_bf16, const float* bias, void* out,
                     unsigned long long* gn_bins, int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit,
                     void* stream) {
-    if (wide) {
+    const bool wide = mode == DbgConv::WIDE;
+    if (mode == DbgConv::DOWN) {
+        if (stride != 2) return fail(nullptr, "%s: stride must be 2 (got %d)", who, stride);
+        if (side % 2 != 0 || !conv_out_side_ok(side / 2))
+            return fail(nullptr, "%s: side must be 8, 16, 32, 64, 128, 256 or 512 (got %d)", who, side);
+        if (B < 1 || (long long)B * (side / 2) * (side / 2) > INT32_MAX)
+            return fail(nullptr, "%s: B must be >= 1 and B * (side / 2)^2 below 2^31 output pixels (got B %d)", who, B);
+    } else if (wide) {
         if (side != 256 && side != 512) return fail(nullptr, "%s: side must be 256 or 512 (got %d)", who, side);
         if (stride != 1) return fail(nullptr, "%s: stride must be 1 (got %d)", who, stride);
         if (B < 1 || (long long)B * side * side > INT32_MAX)
@@ -1577,7 +1588,7 @@ static int dbg_conv(const char* who, bool wide, const void* x_bf16, const void* 
     return dbg_run([&](lfm_ctx* ctx) {
         UNetState u;
         if (!push_conv(&u, B, static_cast<const __nv_bfloat16*>(x_bf16), side, Cin, stride, static_cast<const __nv_bfloat16*>(w_bf16),
-                       bias, Cout, out, epi))
+                       bias, Cout, out, epi, mode == DbgConv::DOWN ? 0 : 1))
             return fail(ctx, "%s: tensor map encode failed", who);
         UOp& o = u.prog[0];
         if (ksplit >= 1) {
@@ -1601,15 +1612,24 @@ static int dbg_conv(const char* who, bool wide, const void* x_bf16, const void* 
 
 extern "C" int lfm_dbg_conv(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins, int B,
                             int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
-    return dbg_conv("lfm_dbg_conv", false, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream);
+    return dbg_conv("lfm_dbg_conv", DbgConv::CONV, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit, stream);
 }
 
 // Stride-1 3x3 convolutions whose output rows are wider than one 128-pixel tile (the row-segment tiles of the VAE decoder's
 // last stages): the same push_conv / run_gemm_op path, never split along K.
 extern "C" int lfm_dbg_conv_wide(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins,
                                  int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
-    return dbg_conv("lfm_dbg_conv_wide", true, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi, ksplit,
-                    stream);
+    return dbg_conv("lfm_dbg_conv_wide", DbgConv::WIDE, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi,
+                    ksplit, stream);
+}
+
+// The VAE encoder's Downsample2D(padding=0): F.pad(x, (0, 1, 0, 1)) then a 3x3 stride-2 convolution, as the network runs it (tap
+// origin 0, the extra bottom row and right column read as the tensor map's zero fill; output rows wider than 128 pixels on
+// row segments).  Arguments as lfm_dbg_conv, checked before the device is touched.
+extern "C" int lfm_dbg_conv_down(const void* x_bf16, const void* w_bf16, const float* bias, void* out, unsigned long long* gn_bins,
+                                 int B, int side, int Cin, int Cout, int stride, int block_n, int epi, int ksplit, void* stream) {
+    return dbg_conv("lfm_dbg_conv_down", DbgConv::DOWN, x_bf16, w_bf16, bias, out, gn_bins, B, side, Cin, Cout, stride, block_n, epi,
+                    ksplit, stream);
 }
 
 // The network's conv_in (input_blocks.0 / conv_in) on the channel concatenation [a | b] of two NCHW fp32 sources.
@@ -1618,9 +1638,11 @@ extern "C" int lfm_dbg_conv_in(const float* a, int a_ch, long long a_stride, con
     if (a_ch < 1 || b_ch < 0 || a_ch + b_ch < 3 || a_ch + b_ch > kConvInMaxChannels)
         return fail(nullptr, "lfm_dbg_conv_in: a_ch >= 1, b_ch >= 0 and a_ch + b_ch in [3, %d] (got %d, %d)", kConvInMaxChannels, a_ch,
                     b_ch);
-    if (side < 1 || side > 256 || conv_in_smem_bytes(a_ch + b_ch, side) > 48 * 1024)
-        return fail(nullptr, "lfm_dbg_conv_in: side must be in [1, 256] with a_ch + b_ch rows of side + 4 floats in 48 KB of shared "
-                             "memory (got side %d, %d channels)", side, a_ch + b_ch);
+    // sides up to 256 for the UNets' latents; 512 for the 3-channel image input of the VAE encoder
+    const bool side_ok = (side >= 1 && side <= 256) || (side == 512 && a_ch + b_ch == 3);
+    if (!side_ok || conv_in_smem_bytes(a_ch + b_ch, side) > 48 * 1024)
+        return fail(nullptr, "lfm_dbg_conv_in: side must be in [1, 256], or 512 with 3 channels, with a_ch + b_ch rows of side + 4 "
+                             "floats in 48 KB of shared memory (got side %d, %d channels)", side, a_ch + b_ch);
     if (a_stride < (long long)a_ch * side * side || (b_ch > 0 && b_stride < (long long)b_ch * side * side))
         return fail(nullptr, "lfm_dbg_conv_in: a_stride / b_stride must hold a_ch / b_ch channels of side^2 floats (got %lld, %lld)",
                     a_stride, b_stride);
@@ -1631,6 +1653,21 @@ extern "C" int lfm_dbg_conv_in(const float* a, int a_ch, long long a_stride, con
     return dbg_run([&](lfm_ctx* ctx) {
         COUNT_LAUNCH(launch_conv_in(static_cast<cudaStream_t>(stream), ConvInSrc{a, a_ch, a_stride}, ConvInSrc{b, b_ch, b_stride}, B, B,
                                     w, bias, out, side, Cout));
+        return 0;
+    });
+}
+
+// The VAE encoder's tail, vae_quant_kernel: quant_conv (8 -> 8) of conv_out's NHWC fp32 [B * HW, 8] output, then mean and the
+// clamped logvar, NCHW fp32 [B, 4, HW].
+extern "C" int lfm_dbg_vae_quant(const float* in, const float* w, const float* bias, float* mean, float* logvar, int B, int HW,
+                                 void* stream) {
+    if (B < 1 || HW < 1 || (long long)B * HW > INT32_MAX)
+        return fail(nullptr, "lfm_dbg_vae_quant: B and HW must be >= 1 with B * HW < 2^31 (got %d, %d)", B, HW);
+    if (in == nullptr || w == nullptr || bias == nullptr || mean == nullptr || logvar == nullptr || !aligned16(in))
+        return fail(nullptr, "lfm_dbg_vae_quant: in, w, bias, mean and logvar must not be NULL (in 16-byte aligned)");
+    return dbg_run([&](lfm_ctx* ctx) {
+        LAUNCH_K(vae_quant_kernel, dim3(blocks_for((size_t)B * HW)), 256, 0, static_cast<cudaStream_t>(stream), in, w, bias, mean, logvar,
+                 B, HW);
         return 0;
     });
 }

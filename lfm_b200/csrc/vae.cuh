@@ -1,6 +1,7 @@
-// lfm_b200 - kernels of the native VAE decode (Stable-Diffusion AutoencoderKL decoder; reference call site
-// test_flow_latent.py:193 `first_stage_model.decode(fake_sample / args.scale_factor).sample`) that are not the shared
-// implicit-GEMM convolution / GroupNorm kernels of unet.cuh, and the device side of the generation loop's
+// lfm_b200 - kernels of the native VAE decode and encode (Stable-Diffusion AutoencoderKL; reference call sites
+// test_flow_latent.py:193 `first_stage_model.decode(fake_sample / args.scale_factor).sample` and
+// downstream_tasks/test_flow_latent_inpainting.py:147 `first_stage_model.encode(masked_image).latent_dist`) that are not the
+// shared implicit-GEMM convolution / GroupNorm kernels of unet.cuh, and the device side of the generation loop's
 // post-processing (test_flow_latent_ddp.py:131-135).
 #pragma once
 #include "common.cuh"
@@ -21,6 +22,30 @@ __global__ void vae_post_quant_kernel(const float* __restrict__ z, const float* 
 #pragma unroll
     for (int o = 0; o < 4; ++o)
         op[static_cast<size_t>(o) * HW] = fmaf(W[o * 4 + 3], v3, fmaf(W[o * 4 + 2], v2, fmaf(W[o * 4 + 1], v1, fmaf(W[o * 4], v0, bias[o]))));
+}
+
+// AutoencoderKL.encode's tail: quant_conv (1x1, 8 -> 8) on the encoder's conv_out, NHWC fp32 [B*HW, 8], then the moments of
+// DiagonalGaussianDistribution: mean = channels 0..3 and logvar = clamp(channels 4..7, -30, 20), both NCHW fp32 [B, 4, HW].
+// Each output is the bias plus the channels in order, one fma each.
+__global__ void vae_quant_kernel(const float* __restrict__ in /*[B*HW, 8]*/, const float* __restrict__ W /*[8][8]*/,
+                                 const float* __restrict__ bias, float* __restrict__ mean, float* __restrict__ logvar, int B, int HW) {
+    pdl_wait();
+    pdl_trigger();
+    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= static_cast<size_t>(B) * HW) return;
+    const float4 lo = *reinterpret_cast<const float4*>(in + i * 8), hi = *reinterpret_cast<const float4*>(in + i * 8 + 4);
+    const float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    const size_t b = i / HW, p = i % HW;
+#pragma unroll
+    for (int o = 0; o < 8; ++o) {
+        float acc = bias[o];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc = fmaf(W[o * 8 + c], v[c], acc);
+        if (o < 4)
+            mean[(b * 4 + o) * HW + p] = acc;
+        else
+            logvar[(b * 4 + o - 4) * HW + p] = fminf(fmaxf(acc, -30.0f), 20.0f);
+    }
 }
 
 // Row softmax of the mid-block attention: P = softmax(S * scale) over the last dimension, S fp32 [R, 128 NV] (the

@@ -92,6 +92,10 @@ class _NativeNet(nn.Module):
     def _create_ctx(self, lib, dev_index):  # -> ctypes handle
         raise NotImplementedError
 
+    def _native_state_dict(self):
+        """The entries uploaded to the native context (lfm_set_param, strict on both sides)."""
+        return self.state_dict()
+
     def _finalize_rows(self, rows: int) -> int:
         """Rows the native workspace is sized for when a context is (re)created for `rows`."""
         return max(rows, self.max_batch_hint or 0)
@@ -114,7 +118,7 @@ class _NativeNet(nn.Module):
         self._release()
         ctx = self._create_ctx(lib, dev_index)
         try:
-            for key, p in self.state_dict().items():
+            for key, p in self._native_state_dict().items():
                 t = p.detach().to(torch.float32).contiguous()
                 shape = (C.c_int64 * t.dim())(*t.shape)
                 _lib.check(lib.lfm_set_param(ctx, key.encode(), C.c_void_p(t.data_ptr()), 0, shape, t.dim()), ctx)

@@ -1,14 +1,17 @@
 """H100-native decoder of the Stable-Diffusion ``AutoencoderKL`` - the VAE decode step of the sampling path
 (``first_stage_model.decode(fake_sample / args.scale_factor).sample``, test_flow_latent.py:131,193;
-test_flow_latent_ddp.py:57,110).
+test_flow_latent_ddp.py:57,110) - and, with ``with_encoder=True``, its encoder (the inpainting loop's
+``first_stage_model.encode(masked_image).latent_dist.sample()``, downstream_tasks/test_flow_latent_inpainting.py:147).
 
 ``diffusers`` is a third-party dependency of the reference that is absent from this image, so this class mirrors the
 part of its interface the reference uses: ``AutoencoderKL.from_pretrained(dir)`` (a LOCAL diffusers-format directory:
 ``config.json`` + ``diffusion_pytorch_model.safetensors`` / ``.bin``; there is no network here), ``.to(device)``,
-``.decode(z).sample``.  Parameters live in an ``nn.Module`` tree with the diffusers ``state_dict`` keys of the decoder
-(``decoder.*``, ``post_quant_conv.*``; a full checkpoint's ``encoder.*`` / ``quant_conv.*`` entries are ignored, legacy
-attention names are renamed as diffusers does); the compute is liblfm_b200.so (``lfm_create_vae`` / ``lfm_decode``:
-wgmma implicit-GEMM convolutions, fused GroupNorm + SiLU, tensor-core attention GEMMs).  ``decode_to_uint8`` also
+``.decode(z).sample``, ``.encode(x).latent_dist``.  Parameters live in an ``nn.Module`` tree with the diffusers
+``state_dict`` keys of the decoder (``decoder.*``, ``post_quant_conv.*``; by default a full checkpoint's ``encoder.*`` /
+``quant_conv.*`` entries are ignored) and, with ``with_encoder=True``, of the encoder too; legacy attention names are
+renamed as diffusers does.  The compute is liblfm_b200.so: ``lfm_create_vae`` / ``lfm_decode`` and
+``lfm_create_vae_encoder`` / ``lfm_encode``, two native contexts that each hold their own half of the weights
+(wgmma implicit-GEMM convolutions, fused GroupNorm + SiLU, tensor-core attention GEMMs).  ``decode_to_uint8`` also
 fuses the generation loop's post-processing (test_flow_latent_ddp.py:131-135).  No PyTorch forward, no fallback.
 """
 from __future__ import annotations
@@ -26,6 +29,8 @@ from . import _lib
 from .network import _Holder, _NativeNet
 
 LEGACY_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
+DECODER_PREFIXES = ("decoder.", "post_quant_conv.")
+ENCODER_PREFIXES = ("encoder.", "quant_conv.")
 
 
 def _resnet(cin, cout):
@@ -49,18 +54,119 @@ class _List(nn.Module):
         return getattr(self, str(i))
 
 
+def _mid_block(c):
+    """UNetMidBlock2D of the decoder and the encoder: resnets.0, attentions.0 (one head of c channels), resnets.1."""
+    mid = _Holder()
+    att = _Holder()
+    att.group_norm = nn.GroupNorm(32, c, eps=1e-6)
+    att.to_q = nn.Linear(c, c)
+    att.to_k = nn.Linear(c, c)
+    att.to_v = nn.Linear(c, c)
+    att.to_out = _List([nn.Linear(c, c)])
+    mid.attentions = _List([att])
+    mid.resnets = _List([_resnet(c, c), _resnet(c, c)])
+    return mid
+
+
+def _encoder(in_channels, boc, layers_per_block, latent_channels):
+    """diffusers ``Encoder`` (double_z): conv_in, down blocks of ResnetBlock2D + Downsample2D(padding=0), the mid block,
+    GroupNorm + SiLU + conv_out to 2 x latent_channels."""
+    enc = _Holder()
+    enc.conv_in = nn.Conv2d(in_channels, boc[0], 3, padding=1)
+    downs, ch = [], boc[0]
+    for i, out in enumerate(boc):
+        blk = _Holder()
+        res = []
+        for _ in range(layers_per_block):
+            res.append(_resnet(ch, out))
+            ch = out
+        blk.resnets = _List(res)
+        if i != len(boc) - 1:
+            down = _Holder()
+            down.conv = nn.Conv2d(ch, ch, 3, stride=2, padding=0)
+            blk.downsamplers = _List([down])
+        downs.append(blk)
+    enc.down_blocks = _List(downs)
+    enc.mid_block = _mid_block(ch)
+    enc.conv_norm_out = nn.GroupNorm(32, ch, eps=1e-6)
+    enc.conv_out = nn.Conv2d(ch, 2 * latent_channels, 3, padding=1)
+    return enc
+
+
+class DiagonalGaussianDistribution:
+    """diffusers ``DiagonalGaussianDistribution`` built from the moments the native encoder returns (logvar already clamped
+    to [-30, 20]): ``std = exp(0.5 logvar)``, ``var = exp(logvar)``, ``sample(generator) = mean + std * eps``, ``mode() = mean``."""
+
+    def __init__(self, mean, logvar):
+        self.mean, self.logvar = mean, logvar
+        self.std = torch.exp(0.5 * logvar)
+        self.var = torch.exp(logvar)
+
+    def sample(self, generator=None):
+        """eps is drawn as diffusers' ``randn_tensor`` draws it: on the generator's device (the mean's when no generator is
+        given), then moved to the mean's device.  On a CUDA generator the CUDA RNG stream advances exactly as under diffusers."""
+        gen_dev = generator.device if generator is not None else self.mean.device
+        eps = torch.randn(self.mean.shape, generator=generator, device=gen_dev, dtype=self.mean.dtype).to(self.mean.device)
+        return self.mean + self.std * eps
+
+    def mode(self):
+        return self.mean
+
+
+class _EncoderNative(_NativeNet):
+    """The encoder's native context (lfm_create_vae_encoder): holds the AutoencoderKL's ``encoder`` and ``quant_conv``
+    modules (shared, not copied), so its upload walks exactly their 108 keys.  Not a registered child of the AutoencoderKL."""
+
+    def __init__(self, vae):
+        super().__init__()
+        self.encoder = vae.encoder
+        self.quant_conv = vae.quant_conv
+        self.block_out_channels, self.layers_per_block = vae.block_out_channels, vae.layers_per_block
+        self.latent_channels, self.in_channels, self.norm_num_groups = vae.latent_channels, vae.in_channels, vae.norm_num_groups
+        self.chunk_rule = vae.decode_chunk
+        self._init_native()
+        self._image_side = None
+
+    def invalidate(self):
+        """The AutoencoderKL's parameters may have changed or moved: redo the version walk on the next call."""
+        self._dirty = True
+        object.__setattr__(self, "_probe_cache", None)
+
+    def latent_side(self):
+        return self._image_side // 2 ** (len(self.block_out_channels) - 1)
+
+    def _version(self):
+        return (self._image_side,) + super()._version()
+
+    def _create_ctx(self, lib, dev_index):
+        boc = self.block_out_channels
+        d = _lib.VaeDesc(self.latent_side(), self.latent_channels, self.in_channels, len(boc), (C.c_int32 * 8)(*boc),
+                         self.layers_per_block, self.norm_num_groups)
+        ctx = C.c_void_p()
+        _lib.check(lib.lfm_create_vae_encoder(C.byref(d), dev_index, C.byref(ctx)))
+        return ctx
+
+    def _finalize_rows(self, rows):
+        return max(rows, self.chunk_rule(self.latent_side()))
+
+
 class AutoencoderKL(_NativeNet):
-    """Decoder-only mirror of ``diffusers.AutoencoderKL`` (defaults = the stabilityai/sd-vae-ft-mse config)."""
+    """Mirror of ``diffusers.AutoencoderKL`` (defaults = the stabilityai/sd-vae-ft-mse config): the decoder, and with
+    ``with_encoder=True`` the encoder as well (248 state-dict keys instead of 140)."""
 
     def __init__(self, in_channels=3, out_channels=3, block_out_channels=(128, 256, 512, 512), layers_per_block=2,
-                 latent_channels=4, norm_num_groups=32, scaling_factor=0.18215, max_batch=16, **unused):
+                 latent_channels=4, norm_num_groups=32, scaling_factor=0.18215, max_batch=16, with_encoder=False, **unused):
         super().__init__()
         self.block_out_channels = tuple(int(c) for c in block_out_channels)
         self.layers_per_block, self.latent_channels, self.out_channels = int(layers_per_block), int(latent_channels), int(out_channels)
+        self.in_channels = int(in_channels)
         self.norm_num_groups = int(norm_num_groups)
+        self.with_encoder = bool(with_encoder)
         self.config = types.SimpleNamespace(scaling_factor=scaling_factor, block_out_channels=self.block_out_channels,
                                             layers_per_block=self.layers_per_block, latent_channels=self.latent_channels)
         self.max_batch_hint = max_batch
+        if self.with_encoder:       # diffusers' registration order: encoder, decoder, quant_conv, post_quant_conv
+            self.encoder = _encoder(self.in_channels, self.block_out_channels, self.layers_per_block, self.latent_channels)
         rev = self.block_out_channels[::-1]
         dec = _Holder()
         dec.conv_in = nn.Conv2d(latent_channels, rev[0], 3, padding=1)
@@ -78,31 +184,31 @@ class AutoencoderKL(_NativeNet):
                 blk.upsamplers = _List([up])
             ups.append(blk)
         dec.up_blocks = _List(ups)
-        mid = _Holder()
-        att = _Holder()
-        att.group_norm = nn.GroupNorm(32, rev[0], eps=1e-6)
-        att.to_q = nn.Linear(rev[0], rev[0])
-        att.to_k = nn.Linear(rev[0], rev[0])
-        att.to_v = nn.Linear(rev[0], rev[0])
-        att.to_out = _List([nn.Linear(rev[0], rev[0])])
-        mid.attentions = _List([att])
-        mid.resnets = _List([_resnet(rev[0], rev[0]), _resnet(rev[0], rev[0])])
-        dec.mid_block = mid
+        dec.mid_block = _mid_block(rev[0])
         dec.conv_norm_out = nn.GroupNorm(32, ch, eps=1e-6)
         dec.conv_out = nn.Conv2d(ch, out_channels, 3, padding=1)
         self.decoder = dec
+        if self.with_encoder:
+            self.quant_conv = nn.Conv2d(2 * latent_channels, 2 * latent_channels, 1)
         self.post_quant_conv = nn.Conv2d(latent_channels, latent_channels, 1)
         self.requires_grad_(False)
         self._init_native()
         self._latent_size = None
+        # the encoder's own native context, not a registered child: the AutoencoderKL's state_dict is not doubled
+        object.__setattr__(self, "_enc_native", _EncoderNative(self) if self.with_encoder else None)
 
     # -- loading ------------------------------------------------------------------------------------------------------
     @staticmethod
     def decoder_state_dict(sd):
-        """The entries of a (possibly full, possibly legacy-named) AutoencoderKL checkpoint this module holds."""
+        """The decoder entries of a (possibly full, possibly legacy-named) AutoencoderKL checkpoint."""
+        return AutoencoderKL._select(sd, DECODER_PREFIXES)
+
+    @staticmethod
+    def _select(sd, prefixes):
+        """The entries of `sd` under `prefixes`, legacy attention names renamed as diffusers does."""
         out = {}
         for k, v in sd.items():
-            if not (k.startswith("decoder.") or k.startswith("post_quant_conv.")):
+            if not k.startswith(prefixes):
                 continue
             parts = k.split(".")
             if "attentions" in parts and len(parts) >= 2 and parts[-2] in LEGACY_ATTN:
@@ -113,11 +219,31 @@ class AutoencoderKL(_NativeNet):
         return out
 
     def load_state_dict(self, state_dict, strict=True, **kw):
-        return super().load_state_dict(self.decoder_state_dict(state_dict), strict=strict, **kw)
+        prefixes = DECODER_PREFIXES + (ENCODER_PREFIXES if self.with_encoder else ())
+        r = super().load_state_dict(self._select(state_dict, prefixes), strict=strict, **kw)
+        self._invalidate_encoder()
+        return r
+
+    def _invalidate_encoder(self):
+        if getattr(self, "_enc_native", None) is not None:
+            self._enc_native.invalidate()
+
+    def mark_dirty(self):
+        super().mark_dirty()
+        self._invalidate_encoder()
+
+    def _apply(self, fn, *a, **k):
+        r = super()._apply(fn, *a, **k)
+        self._invalidate_encoder()
+        return r
+
+    def _native_state_dict(self):
+        return self.decoder_state_dict(self.state_dict())
 
     @classmethod
-    def from_pretrained(cls, path, subfolder=None, **kwargs):
-        """``AutoencoderKL.from_pretrained`` for a LOCAL diffusers directory (no hub access in this environment)."""
+    def from_pretrained(cls, path, subfolder=None, with_encoder=False, **kwargs):
+        """``AutoencoderKL.from_pretrained`` for a LOCAL diffusers directory (no hub access in this environment).
+        ``with_encoder=True`` also loads the encoder (strictly: every ``encoder.*`` / ``quant_conv.*`` key must be there)."""
         root = os.path.join(path, subfolder) if subfolder else path
         cfg_path = os.path.join(root, "config.json")
         if not os.path.isfile(cfg_path):
@@ -128,7 +254,7 @@ class AutoencoderKL(_NativeNet):
             cfg = json.load(f)
         keep = ("in_channels", "out_channels", "block_out_channels", "layers_per_block", "latent_channels", "norm_num_groups",
                 "scaling_factor")
-        vae = cls(**{k: cfg[k] for k in keep if k in cfg}, **kwargs)
+        vae = cls(**{k: cfg[k] for k in keep if k in cfg}, with_encoder=with_encoder, **kwargs)
         st = os.path.join(root, "diffusion_pytorch_model.safetensors")
         if os.path.isfile(st):
             from safetensors.torch import load_file
@@ -192,8 +318,40 @@ class AutoencoderKL(_NativeNet):
         in one pass: [B, 4, s, s] latents -> [B, 8s, 8s, 3] uint8 on the device."""
         return self._decode_native(z, False, True)[1]
 
+    # -- first_stage_model.encode(x).latent_dist  (downstream_tasks/test_flow_latent_inpainting.py:147) ----------------------
+    def encode(self, x, return_dict=True):
+        """x fp32 [B, 3, S, S] on a CUDA device (S = 128, 256 or 512) -> ``.latent_dist``, a DiagonalGaussianDistribution over
+        [B, 4, S / 8, S / 8] latents (``(latent_dist,)`` with ``return_dict=False``).  Runs in chunks of ``decode_chunk``
+        images, the decoder's rule at the same latent side."""
+        if not self.with_encoder:
+            raise RuntimeError("this AutoencoderKL holds the decoder only: build it with with_encoder=True "
+                               "(AutoencoderKL(..., with_encoder=True) / from_pretrained(path, with_encoder=True))")
+        if not x.is_cuda:
+            raise RuntimeError("lfm_b200: x must be a CUDA tensor (no CPU path)")
+        x = x.to(torch.float32).contiguous()
+        B, Cc, h, w = x.shape
+        down = 2 ** (len(self.block_out_channels) - 1)
+        if Cc != self.in_channels or h != w or h % down != 0:
+            raise ValueError(f"expected square images [B, {self.in_channels}, S, S] with S a multiple of {down}, got {tuple(x.shape)}")
+        enc = self._enc_native
+        if enc._image_side != h:
+            enc._image_side = h
+            enc.invalidate()                  # another image size = another native context
+        s = h // down
+        mean = torch.empty(B, self.latent_channels, s, s, device=x.device)
+        logvar = torch.empty_like(mean)
+        chunk = self.decode_chunk(s)
+        ctx = enc.native(min(B, chunk), x.device)
+        lib = _lib.load()
+        for i in range(0, B, chunk):
+            n = min(chunk, B - i)
+            _lib.check(lib.lfm_encode(ctx, x[i:i + n].data_ptr(), n, mean[i:i + n].data_ptr(), logvar[i:i + n].data_ptr(),
+                                      self._stream(x.device)), ctx)
+        dist = DiagonalGaussianDistribution(mean, logvar)
+        return types.SimpleNamespace(latent_dist=dist) if return_dict else (dist,)
+
     def forward(self, *a, **k):
-        raise NotImplementedError("only the decoder of the AutoencoderKL is on the sampling path: use .decode(z)")
+        raise NotImplementedError("the native AutoencoderKL has no forward: use .decode(z) (and .encode(x) with with_encoder=True)")
 
     def decode_flops_per_image(self, latent_side: int = 32) -> float:
         """Algorithmic FLOPs (2 x MAC) of one decode: the convolutions, the four attention projections and the two
@@ -216,9 +374,27 @@ class AutoencoderKL(_NativeNet):
         fl += 2.0 * side * side * 9 * ch * self.out_channels
         return fl
 
+    def encode_flops_per_image(self, image_side: int = 256) -> float:
+        """Algorithmic FLOPs (2 x MAC) of one encode: the convolutions, quant_conv, the four attention projections and the
+        two attention GEMMs."""
+        boc, L2 = self.block_out_channels, 2 * self.latent_channels
+        side, ch = image_side, boc[0]
+        fl = 2.0 * side * side * 9 * self.in_channels * ch
+        for i, out in enumerate(boc):
+            px = side * side
+            for _ in range(self.layers_per_block):
+                fl += 2.0 * px * 9 * (ch * out + out * out) + (2.0 * px * ch * out if ch != out else 0.0)
+                ch = out
+            if i != len(boc) - 1:
+                side //= 2
+                fl += 2.0 * side * side * 9 * ch * ch
+        px = side * side
+        fl += 2 * (2.0 * px * 9 * 2 * ch * ch) + 2.0 * px * 4 * ch * ch + 4.0 * px * px * ch        # mid block
+        return fl + 2.0 * px * (9 * ch * L2 + L2 * L2)
+
 
 def synthetic_vae_state_dict(vae: AutoencoderKL, seed: int = 1):
-    """Seeded non-degenerate decoder weights (the real sd-vae-ft-mse file is a network download): conv / linear
+    """Seeded non-degenerate weights for every key of `vae` (the decoder's, and the encoder's with with_encoder=True) (the real sd-vae-ft-mse file is a network download): conv / linear
     U(-a, a) with a = 1/sqrt(fan_in); GroupNorm weight 1 + 0.1 N, bias 0.1 N; biases 0.02 N.  Every tensor has its own
     generator seeded from (seed, crc32(key)), so the result does not depend on the key order; same recipe as
     oracle.vae.synthetic_state_dict (tests/test_host_logic.py checks they agree)."""
