@@ -158,6 +158,18 @@ int lfm_create_vae_encoder(const lfm_vae_desc* desc, int device, lfm_ctx** out);
  * An lfm_create_vae context refuses this call; an lfm_create_vae_encoder context refuses lfm_decode. */
 int lfm_encode(lfm_ctx* ctx, const float* x, int B, float* mean, float* logvar, void* stream);
 
+/* The semantic-synthesis condition, cond_stage_model(one_hot(seg, num_cls).permute(0, 3, 1, 2).float())
+ * (downstream_tasks/test_flow_latent_semantic_syn.py:94,131-135; models/encoder.py:90 SpatialRescaler with n_stages halvings,
+ * method "bilinear", multiplier 0.5 and a bias-free 1x1 channel_mapper), computed from the labels without the one-hot:
+ *   labels: [B, H, W] uint8 (device); H and W multiples of f = 2^n_stages, B * H * W < 2^31
+ *   weight: [out_ch, num_classes] fp32 (channel_mapper.weight)
+ *   out:    [B, out_ch, H / f, W / f] fp32 NCHW, out[b, k, i, j] = sum_c weight[k, c] * n_c / f^2 with n_c the count of class c
+ *           in the label block [f i, f i + f) x [f j, f j + f), accumulated with one fmaf per class in class order.
+ * 1 <= num_classes <= 256, 1 <= out_ch <= 16, 0 <= n_stages <= 4.  Labels >= num_classes are not counted (the caller validates
+ * them).  No context: the work runs on the current device, stream-ordered on `stream`; errors through lfm_last_error(NULL). */
+int lfm_label_condition(const uint8_t* labels, int B, int H, int W, int num_classes, int n_stages, const float* weight, int out_ch,
+                        float* out, void* stream);
+
 /* nn.Module.load_state_dict (test_flow_latent.py:142): one call per state-dict entry, `key` exactly as in the
  * reference state_dict (SURVEY.md 8(b)); `ptr` may be a host or a device pointer (fp32).  The data is copied
  * (GEMM weights are repacked to bf16).  Unknown key or wrong shape -> error (strict=True behaviour). */

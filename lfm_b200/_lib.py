@@ -48,6 +48,7 @@ SYMBOLS = {
     "lfm_decode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "lfm_create_vae_encoder": (C.c_int, [C.POINTER(VaeDesc), C.c_int, C.POINTER(_P)]),
     "lfm_encode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "lfm_label_condition": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "lfm_set_param": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.POINTER(C.c_int64), C.c_int]),
     "lfm_finalize": (C.c_int, [_P, C.c_int]),
     "lfm_set_condition": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),

@@ -1360,7 +1360,8 @@ extern "C" void lfm_destroy(lfm_ctx* ctx) {
 // kernel-level test entry points
 
 // Runs one kernel-level entry's launches, `op(ctx)`, on the current device, after its arguments are checked.  `ctx` stands in
-// for the network context: it receives the error message and counts the launches.
+// for the network context: it receives the error message and counts the launches.  lfm_label_condition, which needs no
+// context either, runs through it too.
 template <typename Op>
 static int dbg_run(Op&& op) {
     g_num_sms = query_num_sms();
@@ -1763,4 +1764,31 @@ extern "C" int lfm_dbg_tokens(lfm_ctx* ctx, float* out, int B) {
     if (ctx->net != NetKind::DIT) return fail(ctx, "lfm_dbg_tokens: DiT only");
     CUDA_OK(cudaMemcpy(out, ctx->x_tok, (size_t)B * ctx->T * ctx->D * sizeof(float), cudaMemcpyDefault));
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// semantic synthesis: the condition of a batch of label maps (label_condition_kernel)
+
+extern "C" int lfm_label_condition(const uint8_t* labels, int B, int H, int W, int num_classes, int n_stages, const float* weight,
+                                   int out_ch, float* out, void* stream) {
+    if (num_classes < 1 || num_classes > kLabelCondMaxClasses)
+        return fail(nullptr, "lfm_label_condition: num_classes must be in [1, %d] (got %d)", kLabelCondMaxClasses, num_classes);
+    if (out_ch < 1 || out_ch > kLabelCondMaxOut)
+        return fail(nullptr, "lfm_label_condition: out_ch must be in [1, %d] (got %d)", kLabelCondMaxOut, out_ch);
+    if (n_stages < 0 || n_stages > kLabelCondMaxStages)
+        return fail(nullptr, "lfm_label_condition: n_stages must be in [0, %d] (got %d)", kLabelCondMaxStages, n_stages);
+    const int f = 1 << n_stages;
+    if (B < 1 || H < 1 || W < 1 || H % f != 0 || W % f != 0 || (long long)B * H * W > INT32_MAX)
+        return fail(nullptr, "lfm_label_condition: H and W must be positive multiples of 2^n_stages = %d, with B * H * W < 2^31 "
+                             "(got B %d, H %d, W %d)", f, B, H, W);
+    if (labels == nullptr || weight == nullptr || out == nullptr)
+        return fail(nullptr, "lfm_label_condition: labels, weight and out must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        static DevOnce once;
+        CUDA_OK(smem_opt_in(once, label_condition_kernel, label_cond_smem_bytes(kLabelCondMaxClasses, kLabelCondMaxOut)));
+        const int Wo = W >> n_stages, segs = (Wo + kLabelCondPix - 1) / kLabelCondPix;
+        LAUNCH_K(label_condition_kernel, dim3(B * (H >> n_stages) * segs), 256, label_cond_smem_bytes(num_classes, out_ch),
+                 static_cast<cudaStream_t>(stream), labels, weight, out, H, W, num_classes, out_ch, n_stages);
+        return 0;
+    });
 }

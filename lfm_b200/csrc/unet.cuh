@@ -911,4 +911,55 @@ skinny_linear_gen_kernel(const float* __restrict__ W, const float* __restrict__ 
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// The semantic-synthesis condition (downstream_tasks/test_flow_latent_semantic_syn.py:131-135): SpatialRescaler(n_stages,
+// bilinear, multiplier 0.5) and its bias-free 1x1 channel_mapper applied to the one-hot of a uint8 label map, without the
+// one-hot.  A bilinear halving without corner alignment averages neighbour pairs with weights 1/2, so on one-hot input the
+// n_stages halvings are exactly the class counts n_c of each f x f label block over f^2 (f = 2^n_stages), and
+//   out[b, k, i, j] = sum_c w[k, c] * (n_c / f^2),   one fmaf per class in class order (deterministic).
+// One block per kLabelCondPix output pixels of one output row: its f label rows are counted into a shared histogram
+// hist[pixel][class] (row pitch K | 1 words, odd so that the pixels of a warp fall in different banks), then each
+// (channel, pixel) pair is one thread's dot product against the weights staged in shared memory.  Labels >= K are not
+// counted: the caller validates them, the kernel only never lets them index memory.
+constexpr int kLabelCondPix = 32;
+constexpr int kLabelCondMaxClasses = 256, kLabelCondMaxOut = 16, kLabelCondMaxStages = 4;
+
+__host__ __device__ constexpr int label_cond_pitch(int K) { return K | 1; }
+__host__ __device__ constexpr int label_cond_smem_bytes(int K, int O) { return (kLabelCondPix * label_cond_pitch(K) + O * K) * 4; }
+
+__global__ void __launch_bounds__(256)
+label_condition_kernel(const uint8_t* __restrict__ labels, const float* __restrict__ weight /*[O][K]*/, float* __restrict__ out,
+                       int H, int W, int K, int O, int stages) {
+    extern __shared__ int lc_smem[];
+    const int KP = label_cond_pitch(K);
+    int* hist = lc_smem;                                               // [kLabelCondPix][KP]
+    float* ws = reinterpret_cast<float*>(lc_smem + kLabelCondPix * KP);  // [O][K]
+    const int Ho = H >> stages, Wo = W >> stages;
+    const int segs = (Wo + kLabelCondPix - 1) / kLabelCondPix;
+    const int seg = blockIdx.x % segs, i = (blockIdx.x / segs) % Ho, b = blockIdx.x / segs / Ho;
+    const int j0 = seg * kLabelCondPix, np = min(kLabelCondPix, Wo - j0);
+    for (int t = threadIdx.x; t < kLabelCondPix * KP; t += blockDim.x) hist[t] = 0;
+    pdl_wait();
+    pdl_trigger();
+    for (int t = threadIdx.x; t < O * K; t += blockDim.x) ws[t] = weight[t];
+    __syncthreads();
+    const int rows = 1 << stages, cols = np << stages;
+    const uint8_t* src = labels + (static_cast<size_t>(b) * H + (static_cast<size_t>(i) << stages)) * W + (static_cast<size_t>(j0) << stages);
+    for (int t = threadIdx.x; t < rows * cols; t += blockDim.x) {
+        const int r = t / cols, c = t - r * cols;
+        const int l = src[static_cast<size_t>(r) * W + c];
+        if (l < K) atomicAdd(&hist[(c >> stages) * KP + l], 1);
+    }
+    __syncthreads();
+    const float inv = 1.0f / static_cast<float>(rows * rows);  // a power of 2: n_c * inv is exact
+    for (int t = threadIdx.x; t < O * np; t += blockDim.x) {
+        const int k = t / np, p = t - k * np;
+        const int* h = hist + p * KP;
+        const float* w = ws + k * K;
+        float acc = 0.f;
+        for (int c = 0; c < K; ++c) acc = fmaf(w[c], static_cast<float>(h[c]) * inv, acc);
+        out[((static_cast<size_t>(b) * O + k) * Ho + i) * Wo + j0 + p] = acc;
+    }
+}
+
 }  // namespace lfm

@@ -21,6 +21,8 @@ images never leave the GPU:
   through two symmetric eigen-decompositions in fp64: ``Tr sqrt(S1 S2) = sum sqrt(eig(S1^1/2 S2 S1^1/2))``, the same
   number ``scipy.linalg.sqrtm`` gives whenever its result is real, without the complex Schur form and on the GPU.
 * :func:`load_statistics` reads the reference's ``*_stat.npy`` / ``.npz`` files (fid_score.py:231-238).
+* ``python -m lfm_b200.fid PATH PATH --inception_weights FILE`` is ``pytorch_fid/fid_score.py PATH PATH``: FID between two
+  image directories and / or statistics files (fid_score.py:254-295), through the classes above.
 
 Note on parity with a reference run: the reference's number is computed from JPEG-compressed files (quality 75 by PIL's
 default); feeding the uint8 images directly removes that compression from the statistic.  ``test_flow_latent.py
@@ -28,7 +30,9 @@ default); feeding the uint8 images directly removes that compression from the st
 """
 from __future__ import annotations
 
+import argparse
 import os
+import pathlib
 from typing import Dict, Optional, Tuple
 
 import numpy as np
@@ -366,3 +370,67 @@ class FIDAccumulator:
         mu, sigma = self.stats.finalize()
         m2, s2 = load_statistics(real_stats_path)
         return frechet_distance(mu, sigma, m2, s2, device=mu.device)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# FID between two paths (pytorch_fid/fid_score.py:254-295)
+# ---------------------------------------------------------------------------------------------------------------------
+IMAGE_EXTENSIONS = {"bmp", "jpg", "jpeg", "pgm", "png", "ppm", "tif", "tiff", "webp"}   # fid_score.py:95
+
+
+def list_images(path: str):
+    """The images of a directory as fid_score.py:263 takes them: its files (not its subdirectories') with an extension of
+    IMAGE_EXTENSIONS, sorted."""
+    root = pathlib.Path(path)
+    return sorted(f for ext in IMAGE_EXTENSIONS for f in root.glob("*.{}".format(ext)))
+
+
+def statistics_of_path(path: str, net: FIDInception, batch_size: int = 50, device=None) -> Tuple[np.ndarray, np.ndarray]:
+    """fid_score.py:254-265: ``.npz`` / ``.npy`` statistics are read; a directory's images, converted to RGB, go through the
+    network as uint8 batches of ``batch_size`` and are summed by :class:`FIDStatistics`.  The images of a batch must share
+    one size, as the reference's DataLoader collate requires."""
+    from PIL import Image
+    if path.endswith(".npz") or path.endswith(".npy"):
+        return load_statistics(path)
+    if batch_size < 1:
+        raise ValueError(f"batch size must be >= 1, got {batch_size}")
+    stats = FIDStatistics(2048, device)
+    files = list_images(path)
+    for i in range(0, len(files), batch_size):
+        batch = [np.asarray(Image.open(f).convert("RGB")) for f in files[i:i + batch_size]]
+        sizes = sorted({b.shape for b in batch})
+        if len(sizes) > 1:
+            raise ValueError(f"{path}: images of one batch differ in size ({', '.join(f'{h}x{w}' for h, w, _ in sizes)}), "
+                             f"from {files[i].name}")
+        stats.update(net(torch.from_numpy(np.stack(batch)).to(device)))
+    mu, sigma = stats.finalize()
+    return mu.cpu().numpy(), sigma.cpu().numpy()
+
+
+def build_parser():
+    p = argparse.ArgumentParser("python -m lfm_b200.fid", description="FID between two image directories or statistics files")
+    p.add_argument("path", type=str, nargs=2, help="paths to the generated images or to .npz / .npy statistics files")
+    p.add_argument("--inception_weights", type=str, required=True,
+                   help="local copy of pt_inception-2015-12-05-6726825d.pth (there is no download)")
+    p.add_argument("--batch-size", type=int, default=50, help="images per network call")
+    p.add_argument("--device", type=str, default=None, help="cuda, cuda:N or cpu (default: cuda when available)")
+    p.add_argument("--dims", type=int, default=2048, choices=[2048], help="pool3 features (the only ones computed here)")
+    return p
+
+
+def main(argv=None) -> float:
+    args = build_parser().parse_args(argv)
+    for p in args.path:
+        if not os.path.exists(p):
+            raise RuntimeError("Invalid path: %s" % p)
+    device = torch.device(args.device if args.device else ("cuda" if torch.cuda.is_available() else "cpu"))
+    net = FIDInception.from_file(args.inception_weights).to(device).eval()
+    m1, s1 = statistics_of_path(args.path[0], net, args.batch_size, device)
+    m2, s2 = statistics_of_path(args.path[1], net, args.batch_size, device)
+    value = frechet_distance(m1, s1, m2, s2, device=device)
+    print("FID: ", value)
+    return value
+
+
+if __name__ == "__main__":
+    main()
