@@ -264,14 +264,17 @@ int lfm_dbg_patch_embed(const float* x, int x_rows, const float* Wt, const float
  * 8; D a multiple of 128 up to 1536; mod_stride a multiple of 4. */
 int lfm_dbg_final_layer(const float* x, const float* shift, const float* scale, int mod_stride, const float* W, const float* bias,
                         float* v_net, int M, int D, int G, int C, int p, void* stream);
-/* softmax(q k^T / 8) v on a [B*256, 3*D] bf16 qkv buffer in the timm feature order ({q,k,v} * D + head * 64 + c) -> out [B*256, D]
- * bf16.  variant 0: the TMA + wgmma kernel the network runs for 256 tokens; 1: the mma.sync flash kernel.  dbg_s must be NULL. */
-int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s, void* stream);
-/* The mma.sync attention kernels (16 / 64 tokens: whole sequence in registers, ch = 64, 80, 128 or 256; other multiples of 64,
- * e.g. 256 / 1024: keys streamed in chunks of 64, ch = 64 or 80).  qkv [B*T, 3*H*ch] bf16 with HEAD-MAJOR features
- * (head * 3 ch + {q,k,v} * ch + c) -> out [B*T, H*ch] bf16.  Scale head_dim^-1/2 (DiT-XL: ch = 80 is head_dim 72 zero-padded);
- * head_dim 0: ch^-1/2, on 16 / 64 tokens computed by the kernel itself as in the UNets. */
-int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream);
+/* Layouts of the qkv rows of lfm_dbg_attention (row = the 3 heads ch features of one token):
+ *   LFM_QKV_TIMM        {q,k,v} * heads ch + head * ch + c   (timm's Attention, the DiT checkpoints)
+ *   LFM_QKV_HEAD_MAJOR  head * 3 ch + {q,k,v} * ch + c       (guided-diffusion's QKVAttentionLegacy) */
+enum { LFM_QKV_TIMM = 0, LFM_QKV_HEAD_MAJOR = 1 };
+/* One attention as the DiT and UNet programs run it, on the kernel and scale their route table picks for (T, ch, layout):
+ * qkv bf16 [B*T, 3 heads ch] -> out bf16 [B*T, heads ch], softmax(q k^T / sqrt(head_dim)) v per (image, head).
+ * ch is the stored head width; head_dim < ch means heads zero-padded from head_dim to ch channels (DiT-XL: 72 stored as 80),
+ * which only the mma.sync kernels take.  Routes: timm layout: 256 tokens with ch 64 (TMA + wgmma).  Head-major: 16 / 64 tokens
+ * with ch 64, 80, 128 or 256; other multiples of 64 tokens with ch 64 or 80; up to 256 tokens with ch a multiple of 8 up to 256
+ * (SIMT, head_dim = ch).  Other shapes, a bad layout or head_dim, and B or heads < 1 are refused before the device is touched. */
+int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int heads, int ch, int head_dim, int layout, void* stream);
 /* The UNet programs' 3x3 convolution (pad 1) as the implicit GEMM the network runs, built and launched by the network's own code.
  *   x: bf16 NHWC [B, side, side, Cin] (Cin % 64 == 0); stride 1 or 2 (output side side / stride: 4, 8, ..., 256).
  *   w: bf16 [Cout, 9 Cin], K index (r * 3 + s) * Cin + c (lfm_set_param's repacked order); bias: fp32 [Cout]; Cout 4 or % 8 == 0.
@@ -323,9 +326,6 @@ int lfm_dbg_gemm_batched(const void* a_bf16, int a_rows, int a_ld, const void* w
 int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb, const void* src_bf16, const unsigned long long* bins,
                       int max_chunks, const float* gamma, const float* beta, const float* film, int film_stride, int act, float eps,
                       void* out_bf16, float* copy_out, void* raw_out, int B, int HW, void* stream);
-/* The UNet programs' attention (QKVAttentionLegacy): qkv bf16 [B*T, 3C], HEAD-MAJOR (head * 3 ch + {q,k,v} * ch + c, ch = C / heads)
- * -> out bf16 [B*T, C], softmax(q k^T / sqrt(ch)) v, on the kernel the network picks for (T, ch).  Shapes no kernel covers are refused. */
-int lfm_dbg_unet_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int C, int heads, void* stream);
 /* Intermediate activations of the last lfm_forward (fp32 token stream [B*T, D] after all blocks). */
 int lfm_dbg_tokens(lfm_ctx* ctx, float* out, int B);
 

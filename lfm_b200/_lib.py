@@ -38,6 +38,9 @@ class OdeStats(C.Structure):
     _fields_ = [("nfe", C.c_int64), ("accepted", C.c_int64), ("rejected", C.c_int64)]
 
 
+QKV_TIMM, QKV_HEAD_MAJOR = 0, 1   # lfm_dbg_attention's qkv layouts (LFM_QKV_*)
+
+
 # every symbol include/lfm_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -70,8 +73,7 @@ SYMBOLS = {
     "lfm_dbg_dit_condition": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
     "lfm_dbg_patch_embed": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_final_layer": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "lfm_dbg_attention": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
-    "lfm_dbg_attention_mma": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_attention": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv_wide": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_conv_down": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
@@ -81,7 +83,6 @@ SYMBOLS = {
                                        C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_groupnorm": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_float, _P, _P, _P,
                                     C.c_int, C.c_int, _P]),
-    "lfm_dbg_unet_attention": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_tokens": (C.c_int, [_P, _P, C.c_int]),
 }
 

@@ -688,25 +688,42 @@ final_layer_generic_kernel(const float* __restrict__ x, const float* __restrict_
     }
 }
 
-// qkv rows of timm's Attention (out-feature = which * D + head * dh + d, models/DiT.py:120 / SURVEY D6) re-ordered ONCE at upload
-// into the head-major layout (head * 3 dhp + which * dhp + d) that the mma.sync attention kernels read (token grids other than 16 x 16,
-// and head_dim 72).  dhp >= dh is the stored head width: DiT-XL's 72 channels are padded to 80 with zero rows, so q.k^T and P.V are
-// unchanged and the padded output channels are exactly zero; the proj weight gets matching zero columns.
-__global__ void dit_qkv_weight_repack_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int D, int dh, int dhp) {
-    const int heads = D / dh;
-    const size_t n = static_cast<size_t>(3) * heads * dhp * D;
+// Orders of the 3 C qkv rows (C = heads * dh; which = q, k, v).  The first two are also the layouts of lfm_dbg_attention
+// (LFM_QKV_TIMM, LFM_QKV_HEAD_MAJOR).
+//   QKV_TIMM        which * C + head * dh + c      timm's Attention (models/DiT.py:120 / SURVEY D6): the DiT checkpoints
+//   QKV_HEAD_MAJOR  head * 3 dhp + which * dhp + c  what the mma.sync and SIMT attention kernels read; dhp >= dh is the stored
+//                                                   head width, rows c >= dh are zero (DiT-XL's 72 channels padded to 80, so
+//                                                   q.k^T and P.V are unchanged and the padded output channels are exactly zero)
+//   QKV_EDM         head * 3 dh + c * 3 + which     UNetBlock.qkv (EDM.py:277-281), a checkpoint order only
+enum QkvOrder { QKV_TIMM = 0, QKV_HEAD_MAJOR = 1, QKV_EDM = 2 };
+
+// The source row of destination row r when the qkv rows are re-ordered ONCE at upload from order `src` to order `dst`
+// (dhp = dh unless dst is QKV_HEAD_MAJOR); -1: a zero padding row.
+LFM_DEVICE int qkv_src_row(int r, int heads, int dh, int dhp, int src, int dst) {
+    int h, which, c;
+    if (dst == QKV_TIMM) {
+        which = r / (heads * dh), h = (r / dh) % heads, c = r % dh;
+    } else {
+        h = r / (3 * dhp), which = (r % (3 * dhp)) / dhp, c = r % dhp;
+        if (c >= dh) return -1;
+    }
+    return src == QKV_EDM ? h * 3 * dh + c * 3 + which : which * heads * dh + h * dh + c;
+}
+// weight [3 C, K] fp32 -> [3 heads dhp, K] bf16
+__global__ void qkv_weight_reorder_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int K, int heads, int dh, int dhp,
+                                          int src, int dst) {
+    const size_t n = static_cast<size_t>(3) * heads * dhp * K;
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int r = static_cast<int>(i / D), k = static_cast<int>(i % D);
-    const int h = r / (3 * dhp), which = (r % (3 * dhp)) / dhp, d = r % dhp;
-    out[i] = d < dh ? __float2bfloat16(w[static_cast<size_t>(which * D + h * dh + d) * D + k]) : __float2bfloat16(0.f);
+    const int r = qkv_src_row(static_cast<int>(i / K), heads, dh, dhp, src, dst);
+    out[i] = r >= 0 ? __float2bfloat16(w[static_cast<size_t>(r) * K + i % K]) : __float2bfloat16(0.f);
 }
-__global__ void dit_qkv_bias_repack_kernel(const float* __restrict__ b, float* __restrict__ out, int D, int dh, int dhp) {
-    const int heads = D / dh;
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= 3 * heads * dhp) return;
-    const int h = r / (3 * dhp), which = (r % (3 * dhp)) / dhp, d = r % dhp;
-    out[r] = d < dh ? b[which * D + h * dh + d] : 0.f;
+// bias [3 C] -> [3 heads dhp], fp32
+__global__ void qkv_bias_reorder_kernel(const float* __restrict__ b, float* __restrict__ out, int heads, int dh, int dhp, int src, int dst) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 3 * heads * dhp) return;
+    const int r = qkv_src_row(i, heads, dh, dhp, src, dst);
+    out[i] = r >= 0 ? b[r] : 0.f;
 }
 // proj weight [D, D] -> [D, heads * dhp]: input feature head * dh + d moves to column head * dhp + d, zero columns for the padding
 __global__ void dit_proj_weight_pad_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int D, int dh, int dhp) {

@@ -3,6 +3,7 @@
 #include "../../include/lfm_b200.h"
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -150,16 +151,6 @@ static cudaError_t launch_gemm_inst(cudaStream_t s, const CUtensorMap& ta, const
     return launch_k(kern, dim3(grid), kGemmThreads, GemmCfg<BN>::kSmemBytes, s, ta, tb, tc, M, N, K, ep, cg, ksplit, split_row_pitch);
 }
 
-// softmax(q k^T / 8) v for 256 tokens, head_dim 64, timm qkv order (attention_wgmma.cuh); tqkv: box {64, kGemmBoxRows} over [rows, 3 C]
-static cudaError_t launch_attention_wgmma(cudaStream_t s, const CUtensorMap& tqkv, __nv_bfloat16* out, int C, int heads, int samples) {
-    static DevOnce once;
-    if (cudaError_t e = smem_opt_in(once, attention_wgmma_t256_d64, kAttnSmemBytes)) return e;
-    const int items = samples * heads * 2;
-    const int grid = items < g_num_sms ? items : g_num_sms;
-    return launch_k(attention_wgmma_t256_d64, dim3(grid), kAttnThreads, kAttnSmemBytes, s, tqkv, out, C, heads, items,
-                    0.125f * 1.4426950408889634f);
-}
-
 // Tile width: 256 columns, unless N fits in 128 or the 256-wide tiles would leave more than half of the SMs idle (small
 // sampling batches) - then 128, which doubles the tiles of the launch.
 static int pick_block_n(int M, int N) {
@@ -217,6 +208,8 @@ static cudaError_t launch_ln(cudaStream_t s, const float* x, __nv_bfloat16* y, c
 
 static inline unsigned blocks_for(size_t n, int threads = 256) { return static_cast<unsigned>((n + threads - 1) / threads); }
 
+#include "attention_host.inc"
+
 // ------------------------------------------------------------------------------------------------
 // context
 
@@ -226,12 +219,10 @@ enum class Xform {
     BF16,             // cast to bf16
     CONV_BF16,        // conv weight [Co, Ci, kh, kw] -> bf16 [Co, kh, kw, Ci]
     TRANSPOSE_F32,    // fp32 [R, rest] -> [rest, R]
-    EDM_QKV_W,        // EDM qkv weight / bias rows re-ordered (aux0 = head dim, aux1 = target layout, edm_qkv_src_row)
-    EDM_QKV_B,
+    QKV_W,            // qkv weight (bf16) / bias (fp32) rows re-ordered, qkv_src_row: aux = {head dim, its stored width,
+    QKV_B,            //   source order, destination order}
     RESAMPLE_FILTER,  // the constant resample_filter of EDM.py:96-98: validated, not stored
-    DIT_QKV_W,        // DiT qkv weight / bias rows re-ordered head-major for the mma.sync attention kernels
-    DIT_QKV_B,        //   (aux0 = head dim, aux1 = its stored, zero-padded width)
-    DIT_PROJ_PAD,     // DiT proj weight with zero columns for the padded head channels (aux0, aux1 as above)
+    DIT_PROJ_PAD,     // DiT proj weight with zero columns for the padded head channels (aux = {head dim, its stored width})
 };
 
 struct ParamSlot {
@@ -239,7 +230,7 @@ struct ParamSlot {
     std::vector<int64_t> shape;
     size_t numel = 0;
     Xform xform = Xform::F32;
-    int aux0 = 0, aux1 = 0;
+    std::array<int, 4> aux{};
     bool set = false;
 };
 
@@ -264,7 +255,6 @@ struct lfm_ctx {
     int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, Nmod = 0, HW = 0;
     int in_chw = 0, out_chw = 0;  // floats of one image of the network input / of the solver state and the velocity
     int dh = 64, dhp = 64, Dq = 0;  // head_dim, its stored (zero-padded) width and the width H * dhp of the attention tensors
-    bool qkv_head_major = false;    // qkv rows re-ordered head-major (everything but T = 256 with head_dim 64, see lfm_create)
     int max_rows = 0;
     bool finalized = false;
     std::string err;
@@ -287,7 +277,7 @@ struct lfm_ctx {
     __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
     CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
     CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok, tmo_mod;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
-    CUtensorMap tm_qkv_attn;  // qkv as read by the 256-token attention (timm order only)
+    AttnOp attn_op;  // qkv -> attn of every block
 
     // solver state
     cudaStream_t stream = nullptr;
@@ -336,23 +326,22 @@ static size_t numel(const std::vector<int64_t>& shape) {
 }
 
 static void add_param(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, Xform xform = Xform::F32,
-                      int aux0 = 0, int aux1 = 0) {
+                      std::array<int, 4> aux = {}) {
     ParamSlot s;
     s.dst = dst;
     s.numel = numel(shape);
     s.shape = std::move(shape);
     s.xform = xform;
-    s.aux0 = aux0;
-    s.aux1 = aux1;
+    s.aux = aux;
     ctx->params[key] = s;
 }
 
 // A parameter whose storage holds exactly its registered shape: allocate numel(shape) elements and register them.
 template <typename Tp>
 static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::vector<int64_t>& shape, Xform xform = Xform::F32,
-                       int aux0 = 0, int aux1 = 0) {
+                       std::array<int, 4> aux = {}) {
     if (dev_alloc(ctx, p, numel(shape))) return 1;
-    add_param(ctx, key, *p, shape, xform, aux0, aux1);
+    add_param(ctx, key, *p, shape, xform, aux);
     return 0;
 }
 
@@ -433,15 +422,15 @@ static int dit_register(lfm_ctx* ctx) {
         if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
         if (dev_alloc(ctx, &b.b_qkv, 3 * Dq)) return 1;
         if (dev_alloc(ctx, &b.w_proj, (size_t)D * Dq)) return 1;
-        if (ctx->qkv_head_major) {
-            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::DIT_QKV_W, ctx->dh, ctx->dhp);
-            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, Xform::DIT_QKV_B, ctx->dh, ctx->dhp);
+        if (network_qkv_layout(T, ctx->dhp) == QKV_HEAD_MAJOR) {
+            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::QKV_W, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
+            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, Xform::QKV_B, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
         } else {
             add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::BF16);
             add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D});
         }
         if (ctx->dhp != ctx->dh)
-            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::DIT_PROJ_PAD, ctx->dh, ctx->dhp);
+            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::DIT_PROJ_PAD, {ctx->dh, ctx->dhp});
         else
             add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::BF16);
         if (alloc_param(ctx, p + "attn.proj.bias", &b.b_proj, {D}) ||
@@ -491,12 +480,10 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->HW = desc->img_resolution;
     ctx->in_chw = ctx->out_chw = ctx->C * ctx->HW * ctx->HW;
     ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
-    // 256 tokens with head_dim 64 (every released preset) keep the checkpoint's timm qkv order, which the flash kernel reads directly.
-    // Everything else - 16 / 64 / 1024 tokens, head_dim 72 (DiT-XL, stored padded to 80) - stores the qkv rows head-major.
+    // head_dim 72 (DiT-XL) is stored padded to 80 channels; the qkv rows are stored in network_qkv_layout's order
     ctx->dh = desc->hidden_size / desc->num_heads;
     ctx->dhp = ctx->dh == 72 ? 80 : 64;
     ctx->Dq = desc->num_heads * ctx->dhp;
-    ctx->qkv_head_major = (ctx->T != 256 || ctx->dh != 64);
     return finish_create(ctx, dit_register(ctx), out);
 }
 
@@ -539,14 +526,19 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
                                                                   static_cast<int>(s.numel / r0));
                 break;
             }
-            case Xform::EDM_QKV_W:
-                edm_qkv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
-                                                                          static_cast<int>(s.shape[1]), s.aux0, s.aux1);
+            case Xform::QKV_W:
+            case Xform::QKV_B: {  // the destination has 3 heads dhp rows
+                const int dh = s.aux[0], dhp = s.aux[1], heads = static_cast<int>(s.shape[0] / 3) / dh;
+                const int K = static_cast<int>(s.numel / s.shape[0]);
+                const size_t out_n = static_cast<size_t>(3) * heads * dhp * K;
+                if (s.xform == Xform::QKV_W)
+                    qkv_weight_reorder_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), K, heads, dh, dhp,
+                                                                          s.aux[2], s.aux[3]);
+                else
+                    qkv_bias_reorder_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<float*>(s.dst), heads, dh, dhp, s.aux[2],
+                                                                        s.aux[3]);
                 break;
-            case Xform::EDM_QKV_B:
-                edm_qkv_bias_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst),
-                                                                        static_cast<int>(s.shape[0] / 3), s.aux0, s.aux1);
-                break;
+            }
             case Xform::RESAMPLE_FILTER: {
                 float h[4] = {0.f, 0.f, 0.f, 0.f};
                 CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
@@ -554,22 +546,10 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
                     if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
                 break;
             }
-            case Xform::DIT_QKV_W: {  // the destination has 3 * heads * aux1 rows
-                const int Dm = static_cast<int>(s.shape[1]);
-                const size_t out_n = static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1 * Dm;
-                dit_qkv_weight_repack_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
-                break;
-            }
-            case Xform::DIT_QKV_B: {
-                const int Dm = static_cast<int>(s.shape[0] / 3);
-                dit_qkv_bias_repack_kernel<<<blocks_for(static_cast<size_t>(3) * (Dm / s.aux0) * s.aux1), 256>>>(
-                    ctx->staging, static_cast<float*>(s.dst), Dm, s.aux0, s.aux1);
-                break;
-            }
             case Xform::DIT_PROJ_PAD: {
                 const int Dm = static_cast<int>(s.shape[0]);
-                const size_t out_n = static_cast<size_t>(Dm) * (Dm / s.aux0) * s.aux1;
-                dit_proj_weight_pad_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux0, s.aux1);
+                const size_t out_n = static_cast<size_t>(Dm) * (Dm / s.aux[0]) * s.aux[1];
+                dit_proj_weight_pad_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux[0], s.aux[1]);
                 break;
             }
         }
@@ -640,7 +620,7 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, kGemmBoxRows);
-    if (!ctx->qkv_head_major) ok &= make_tmap_bf16(&ctx->tm_qkv_attn, ctx->qkv, M, 3 * Dq, kGemmBoxRows);
+    ok &= attn_plan(&ctx->attn_op, ctx->qkv, ctx->attn, T, ctx->dhp, ctx->dh, ctx->H, network_qkv_layout(T, ctx->dhp), R);
     ok &= make_tmap_out(&ctx->tmo_qkv, ctx->qkv, M, 3 * Dq, 3 * Dq, false);
     ok &= make_tmap_out(&ctx->tmo_hmid, ctx->hmid, M, Hd, Hd, false);
     ok &= make_tmap_out(&ctx->tmo_x_tok, ctx->x_tok, M, D, D, true);
@@ -763,14 +743,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         }
         {
             next_dir();  // attention reads each (sample, head) once: the sweep direction only keeps the GEMMs alternating
-            // head_dim 64 keeps the kernel's own ch^-1/2; the padded DiT-XL heads pass the true head_dim^-1/2
-            const float sc = 1.4426950408889634f / sqrtf(static_cast<float>(ctx->dh));
-            if (!ctx->qkv_head_major)                          // 256 tokens, head_dim 64: TMA + wgmma
-                COUNT_LAUNCH(launch_attention_wgmma(s, ctx->tm_qkv_attn, ctx->attn, Dq, ctx->H, rows));
-            else if (T == 16 || T == 64)                       // 4 x 4 / 8 x 8 token grids: the whole sequence in registers
-                COUNT_LAUNCH(launch_attention_mma(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, ctx->dh == 64 ? 0.f : sc));
-            else                                               // 1024 tokens, head_dim 72: keys streamed in chunks of 64
-                COUNT_LAUNCH(launch_attention_flash(s, ctx->qkv, ctx->attn, T, ctx->dhp, Dq, ctx->H, rows * ctx->H, sc, false));
+            COUNT_LAUNCH(launch_attention(ctx->attn_op, s, rows));
         }
         {
             GemmEpi ep{b.b_proj, ctx->x_tok, D, mb + 2 * D, Nmod, T};  // x += gate_msa * proj(...)   (models/DiT.py:129)
@@ -1493,45 +1466,26 @@ extern "C" int lfm_dbg_final_layer(const float* x, const float* shift, const flo
     });
 }
 
-extern "C" int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int H, int variant, float* dbg_s,
+extern "C" int lfm_dbg_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int heads, int ch, int head_dim, int layout,
                                  void* stream) {
-    if (variant != 0 && variant != 1) return fail(nullptr, "lfm_dbg_attention: variant must be 0 (wgmma) or 1 (mma.sync flash)");
-    if (dbg_s != nullptr) return fail(nullptr, "lfm_dbg_attention: dbg_s is not supported (pass NULL)");
+    if (layout != LFM_QKV_TIMM && layout != LFM_QKV_HEAD_MAJOR)
+        return fail(nullptr, "lfm_dbg_attention: layout must be LFM_QKV_TIMM (0) or LFM_QKV_HEAD_MAJOR (1) (got %d)", layout);
+    if (B < 1 || heads < 1) return fail(nullptr, "lfm_dbg_attention: B and heads must be >= 1 (got B %d, heads %d)", B, heads);
+    if (head_dim < 1 || head_dim > ch) return fail(nullptr, "lfm_dbg_attention: head_dim must be in [1, ch] (got head_dim %d, ch %d)", head_dim, ch);
+    const AttnKernel k = attn_route(T, ch, layout);
+    if (k == AttnKernel::NONE)
+        return fail(nullptr, "lfm_dbg_attention: %d tokens with a head width of %d channels in the %s layout are not supported", T, ch,
+                    layout == LFM_QKV_TIMM ? "timm" : "head-major");
+    if (head_dim < ch && !attn_takes_padded_heads(k))
+        return fail(nullptr, "lfm_dbg_attention: head_dim %d < ch: the kernel for %d tokens with %d channels takes no padded heads", head_dim,
+                    T, ch);
+    if (qkv_bf16 == nullptr || out_bf16 == nullptr) return fail(nullptr, "lfm_dbg_attention: qkv and out must not be NULL");
     return dbg_run([&](lfm_ctx* ctx) {
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        if (variant == 0) {
-            CUtensorMap tq;
-            if (!make_tmap_bf16(&tq, qkv_bf16, (uint64_t)B * 256, (uint64_t)3 * H * 64, kGemmBoxRows))
-                return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
-            CUDA_OK(launch_attention_wgmma(s, tq, static_cast<__nv_bfloat16*>(out_bf16), H * 64, H, B));
-        } else {
-            const float sc = 0.125f * 1.4426950408889634f;  // head_dim^-0.5 * log2(e), head_dim = 64
-            CUDA_OK(launch_attention_flash(s, static_cast<const __nv_bfloat16*>(qkv_bf16), static_cast<__nv_bfloat16*>(out_bf16), 256,
-                                           64, H * 64, H, B * H, sc, true));
-        }
-        return 0;
-    });
-}
-
-extern "C" int lfm_dbg_attention_mma(const void* qkv_bf16, void* out_bf16, int B, int H, int T, int ch, int head_dim, void* stream) {
-    if (!(ch == 64 || ch == 80 || ch == 128 || ch == 256) || head_dim < 0 || head_dim > ch)
-        return fail(nullptr, "lfm_dbg_attention_mma: ch must be 64, 80, 128 or 256 and 0 <= head_dim <= ch (got ch %d, head_dim %d)", ch,
-                    head_dim);
-    const bool short_grid = T == 16 || T == 64;
-    if (!short_grid && !(T > 0 && T % 64 == 0 && (ch == 64 || ch == 80)))
-        return fail(nullptr, "lfm_dbg_attention_mma: T must be 16 or 64, or a multiple of 64 with ch 64 / 80 (got T %d, ch %d)", T, ch);
-    if (B < 1 || H < 1) return fail(nullptr, "lfm_dbg_attention_mma: B and H must be >= 1 (got %d, %d)", B, H);
-    // head_dim 0: the short-grid kernel's own ch^-1/2 (what the UNets run); the flash kernel always takes the scale from the host
-    const float sc = head_dim > 0 ? 1.4426950408889634f / sqrtf(static_cast<float>(head_dim))
-                                  : (short_grid ? 0.f : 1.4426950408889634f / sqrtf(static_cast<float>(ch)));
-    return dbg_run([&](lfm_ctx* ctx) {
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv_bf16);
-        __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out_bf16);
-        if (short_grid)
-            CUDA_OK(launch_attention_mma(s, q, o, T, ch, H * ch, H, B * H, sc));
-        else
-            CUDA_OK(launch_attention_flash(s, q, o, T, ch, H * ch, H, B * H, sc, false));
+        AttnOp op;
+        if (!attn_plan(&op, static_cast<const __nv_bfloat16*>(qkv_bf16), static_cast<__nv_bfloat16*>(out_bf16), T, ch, head_dim, heads,
+                       layout, B))
+            return fail(ctx, "lfm_dbg_attention: tensor map encode failed");
+        CUDA_OK(launch_attention(op, static_cast<cudaStream_t>(stream), B));
         return 0;
     });
 }
@@ -1737,25 +1691,6 @@ extern "C" int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb,
             if (rc == 0 && !o.skip) rc = run_gn_op(ctx, &u, o, s, B, film_stride);
         if (u.partial != nullptr) CUDA_OK(cudaFreeAsync(u.partial, s));
         return rc;
-    });
-}
-
-extern "C" int lfm_dbg_unet_attention(const void* qkv_bf16, void* out_bf16, int B, int T, int C, int heads, void* stream) {
-    if (B < 1 || heads < 1 || C % heads != 0)
-        return fail(nullptr, "lfm_dbg_unet_attention: B and heads must be >= 1 and C a multiple of heads (got B %d, C %d, heads %d)", B, C,
-                    heads);
-    if (!unet_attn_supported(T, C / heads))
-        return fail(nullptr, "lfm_dbg_unet_attention: %d tokens with a head width of %d channels is not supported", T, C / heads);
-    if (qkv_bf16 == nullptr || out_bf16 == nullptr) return fail(nullptr, "lfm_dbg_unet_attention: qkv and out must not be NULL");
-    return dbg_run([&](lfm_ctx* ctx) {
-        UOp o;
-        o.kind = U_ATTN;
-        o.qkv = static_cast<const __nv_bfloat16*>(qkv_bf16);
-        o.att = static_cast<__nv_bfloat16*>(out_bf16);
-        o.HW = T;
-        o.C = C;
-        o.heads = heads;
-        return run_attn_op(ctx, o, static_cast<cudaStream_t>(stream), B);
     });
 }
 

@@ -808,32 +808,6 @@ __global__ void resample2x_kernel(const __nv_bfloat16* __restrict__ a_in, __nv_b
     }
 }
 
-// UNetBlock.qkv rows (EDM.py:277-281: out-channel = head*3dh + c*3 + {q,k,v}) re-ordered at load time into the
-// layout of the attention kernel that will consume them:
-//   mode 0  head*3dh + {q,k,v}*dh + c   (attention_small*_kernel, the guided-diffusion "legacy" order)
-//   mode 1  {q,k,v}*C + head*dh + c     (attention3_t256_d64, the DiT order)
-LFM_DEVICE int edm_qkv_src_row(int r, int C, int dh, int mode) {
-    int h, w, c;
-    if (mode == 0) {
-        h = r / (3 * dh), w = (r % (3 * dh)) / dh, c = r % dh;
-    } else {
-        w = r / C, h = (r % C) / dh, c = r % dh;
-    }
-    return h * 3 * dh + c * 3 + w;
-}
-__global__ void edm_qkv_weight_repack_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int C, int dh, int mode) {
-    const size_t n = static_cast<size_t>(3) * C * C;
-    const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int r = static_cast<int>(i / C), k = static_cast<int>(i % C);
-    out[i] = __float2bfloat16(w[static_cast<size_t>(edm_qkv_src_row(r, C, dh, mode)) * C + k]);
-}
-__global__ void edm_qkv_bias_repack_kernel(const float* __restrict__ b, float* __restrict__ out, int C, int dh, int mode) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= 3 * C) return;
-    out[r] = b[edm_qkv_src_row(r, C, dh, mode)];
-}
-
 // Labels of one network batch for the one-hot column gather of map_label (EDM.py:822-829): row b reads table row
 // y[b]; under forward_with_cfg (drop_half_label) rows >= rows/2 read the all-zero row `null_row`.
 __global__ void edm_labels_kernel(const long long* __restrict__ y, long long* __restrict__ out, int rows, int drop_from, int null_row) {

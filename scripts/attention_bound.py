@@ -44,7 +44,7 @@ s = C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def attn():
-    assert lib.lfm_dbg_attention(C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr()), B, H, 0, None, s) == 0, _lib.last_error()
+    assert lib.lfm_dbg_attention(C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr()), B, T, H, DH, DH, _lib.QKV_TIMM, s) == 0, _lib.last_error()
 
 
 src = torch.empty(512 << 20, dtype=torch.uint8, device=dev)   # 512 MB each way: far beyond the 50 MB L2

@@ -347,52 +347,59 @@ def test_vae_attention_batched_gemms(dev, T, B):
     assert_within(O, ref, bf16_ulp(ref) + dot_c(T) * absref, "O = P V + b")
 
 
-# ------------------------------------------------------------------------------------------------ UNet attention
+# ------------------------------------------------------------------------------------------------ attention
 
 
-def attention_ref(qkv, B, T, heads, ch):
-    """softmax(q k^T / sqrt(ch)) v in fp64 on head-major qkv rows; also P |V| (the scale of the bf16-P rounding)."""
-    q, k, v = qkv.double().reshape(B, T, heads, 3, ch).permute(3, 0, 2, 1, 4)
-    p = torch.softmax((q @ k.transpose(-1, -2)) * ch ** -0.5, -1)
-    o, pa = p @ v, p @ v.abs()
-    return [t.transpose(1, 2).reshape(B * T, heads * ch) for t in (o, pa)]
+def attention_ref(q, k, v, head_dim):
+    """softmax(q k^T / sqrt(head_dim)) v in fp64 on q, k, v [B, T, heads, ch]; also P |V| (the scale of the bf16-P rounding); both
+    [B T, heads ch]."""
+    B, T, H, ch = q.shape
+    q, k, v = (x.double().transpose(1, 2) for x in (q, k, v))   # [B, heads, T, ch]
+    p = torch.softmax((q @ k.transpose(-1, -2)) * head_dim ** -0.5, -1)
+    return [o.transpose(1, 2).reshape(B * T, H * ch) for o in (p @ v, p @ v.abs())]
 
 
-# (T, ch, heads, B): every route of the U_ATTN dispatch
-ATTN_CASES = [
-    (16, 64, 4, 5), (16, 128, 2, 3), (16, 256, 4, 8), (64, 64, 2, 3), (64, 128, 4, 4), (64, 256, 2, 2),   # attention_mma_kernel
-    (256, 64, 4, 2), (1024, 64, 2, 2),                                                                      # flash
-    (16, 32, 4, 3), (16, 96, 2, 3), (64, 32, 4, 2), (64, 96, 2, 3),                                         # SIMT, shared memory
-    (256, 32, 2, 2), (256, 96, 2, 2), (256, 128, 2, 2),
-    (256, 256, 1, 2),                                                                                       # SIMT, plain
-]
+TIMM, HEAD_MAJOR = _lib.QKV_TIMM, _lib.QKV_HEAD_MAJOR
+ATTN_BH = [(1, 1), (2, 4), (3, 12), (64, 16), (5, 16), (7, 6), (33, 12), (128, 16)]
+# (layout, T, ch, head_dim, heads, B): every route of the table, at the shapes the networks run
+ATTN_CASES = (
+    [(TIMM, 256, 64, 64, H, B) for B, H in ATTN_BH]             # TMA + wgmma: the DiT /2 presets, EDM 16 x 16
+    + [(HEAD_MAJOR, 256, 64, 64, H, B) for B, H in ATTN_BH]     # the same data on flash: ADM 16 x 16
+    # DiT geometries outside 256 tokens / head_dim 64: heads zero-padded from 72 to 80 channels, 1024 tokens
+    + [(HEAD_MAJOR, 1024, 64, 64, 4, 2), (HEAD_MAJOR, 256, 80, 72, 16, 3), (HEAD_MAJOR, 256, 64, 64, 3, 2), (HEAD_MAJOR, 64, 80, 72, 16, 5),
+       (HEAD_MAJOR, 16, 80, 72, 16, 7), (HEAD_MAJOR, 128, 80, 72, 2, 1)]
+    # UNet shapes: attention_mma_kernel, flash, SIMT with K / V in shared memory, plain SIMT ((256, 64, 4 heads, B 2) is above)
+    + [(HEAD_MAJOR, T, ch, ch, heads, B) for T, ch, heads, B in [
+        (16, 64, 4, 5), (16, 128, 2, 3), (16, 256, 4, 8), (64, 64, 2, 3), (64, 128, 4, 4), (64, 256, 2, 2), (1024, 64, 2, 2),
+        (16, 32, 4, 3), (16, 96, 2, 3), (64, 32, 4, 2), (64, 96, 2, 3), (256, 32, 2, 2), (256, 96, 2, 2), (256, 128, 2, 2),
+        (256, 256, 1, 2)]]
+    # head_dim = ch on attention_mma_kernel: the kernel's own ch^-1/2, as the UNets run it
+    + [(HEAD_MAJOR, T, ch, ch, 2, 3) for T, ch in [(16, 128), (16, 256), (64, 128), (64, 256), (256, 64)]]
+    # 80-channel UNet heads: attention_mma_kernel and flash
+    + [(HEAD_MAJOR, 64, 80, 80, 4, 3), (HEAD_MAJOR, 256, 80, 80, 4, 2)]
+)
 
 
-@pytest.mark.parametrize("T,ch,heads,B", ATTN_CASES)
-def test_unet_attention(dev, T, ch, heads, B):
-    g = torch.Generator().manual_seed(T * ch + heads + B)
-    qkv = torch.randn(B * T, 3 * heads * ch, generator=g).cuda().bfloat16()
-    ref, pv = attention_ref(qkv, B, T, heads, ch)
+@pytest.mark.parametrize("layout,T,ch,head_dim,heads,B", ATTN_CASES)
+def test_attention(dev, layout, T, ch, head_dim, heads, B):
+    """lfm_dbg_attention (the op and launch the networks run for the shape) against an fp64 reference on the same bf16 q, k, v.
+    Cases that differ only in layout hold the same q, k, v."""
+    g = torch.Generator().manual_seed(B * 1000 + heads * 100 + T + ch)
+    qkv = torch.randn(B, T, 3, heads, ch, generator=g)
+    qkv[..., head_dim:] = 0                                       # the padding channels are zero (zero weight rows)
+    qkv = qkv.to(dev).bfloat16()
+    ref, pv = attention_ref(*qkv.unbind(2), head_dim)
+    rows = qkv if layout == TIMM else qkv.transpose(2, 3)         # {q,k,v} * heads ch + head * ch + c, or head * 3 ch + {q,k,v} * ch + c
+    rows = rows.reshape(B * T, 3 * heads * ch).contiguous()
     out = torch.full((B * T, heads * ch), float("nan"), device=dev).bfloat16()
-    rc = _lib.load().lfm_dbg_unet_attention(P(qkv), P(out), B, T, heads * ch, heads, None)
+    rc = _lib.load().lfm_dbg_attention(P(rows), P(out), B, T, heads, ch, head_dim, layout, None)
     torch.cuda.synchronize()
     assert rc == 0, _lib.last_error()
-    assert_within(out, ref, bf16_ulp(ref) + 2.0 ** -8 * pv, f"attention T {T} ch {ch}")
-
-
-@pytest.mark.parametrize("T,ch", [(16, 128), (16, 256), (64, 128), (64, 256), (256, 64)])
-def test_attention_mma_default_scale(dev, T, ch):
-    """lfm_dbg_attention_mma with head_dim 0 (the kernel's own ch^-1/2, as the UNets call it) and with head_dim = ch."""
-    B, H = 3, 2
-    g = torch.Generator().manual_seed(T + ch)
-    qkv = torch.randn(B * T, 3 * H * ch, generator=g).cuda().bfloat16()
-    ref, pv = attention_ref(qkv, B, T, H, ch)
-    for head_dim in (0, ch):
-        out = torch.full((B * T, H * ch), float("nan"), device=dev).bfloat16()
-        rc = _lib.load().lfm_dbg_attention_mma(P(qkv), P(out), B, H, T, ch, head_dim, None)
-        torch.cuda.synchronize()
-        assert rc == 0, _lib.last_error()
-        assert_within(out, ref, bf16_ulp(ref) + 2.0 ** -8 * pv, f"attention_mma T {T} ch {ch} head_dim {head_dim}")
+    what = f"attention layout {layout} T {T} ch {ch} head_dim {head_dim} heads {heads} B {B}"
+    assert rel_l2(out, ref) < 5e-3, what                          # P and O are rounded to bf16
+    assert_within(out, ref, bf16_ulp(ref) + 2.0 ** -8 * pv, what)
+    if head_dim < ch:
+        assert float(out.float().reshape(B * T, heads, ch)[..., head_dim:].abs().max()) == 0.0   # padded output channels are exactly zero
 
 
 # ------------------------------------------------------------------------------------------------ refusals

@@ -13,8 +13,10 @@ the stored qkv / attention / MLP-hidden activations to bf16:
     tanh.approx term (tests/test_gpu_dit_kernels.py derives them); measured at most 0.011 (fp32), 0.50 (bf16), 0.48 (GELU)
   * attention vs fp64 softmax(q k^T / sqrt(head_dim)) v ............ rel-L2 <= 5e-3; elementwise one bf16 ulp + 2^-8 (P |V|),
     measured at most 0.34 (256 tokens, both kernels) and 0.52 (the mma.sync kernels of the other geometries)
+    (tests/test_gpu_kernels.py test_attention)
 The measured fractions are from an NVIDIA H100 80GB HBM3 at its 700 W power limit.
-The UNet / EDM / VAE kernels are compared op by op in tests/test_gpu_kernels.py, the DiT's in tests/test_gpu_dit_kernels.py.
+The UNet / EDM / VAE kernels and the attention are compared op by op in tests/test_gpu_kernels.py, the DiT's other kernels in
+tests/test_gpu_dit_kernels.py.
 """
 import ctypes as C
 import types
@@ -109,52 +111,6 @@ def test_gemm_epilogues(dev, M, N, K, epi, bn):
     assert rc == 0, _lib.last_error()
     assert rel_l2(out.double().cpu(), ref.cpu()) < tol
     tk.assert_within(out, ref, bound, f"gemm {M}x{N}x{K} epi {epi} bn {bn}")
-
-
-def attention_ref(qkv, head_dim):
-    """softmax(q k^T / sqrt(head_dim)) v in fp64 on bf16 qkv viewed as [B, T, H, {q,k,v}, ch], and P |V| (the scale of the kernels'
-    bf16 rounding of P); both [B T, H ch]."""
-    B, T, H, _, ch = qkv.shape
-    q, k, v = qkv.double().permute(3, 0, 2, 1, 4)    # [B, H, T, ch] each
-    p = torch.softmax((q @ k.transpose(-1, -2)) * head_dim ** -0.5, dim=-1)
-    return [o.transpose(1, 2).reshape(B * T, H * ch) for o in (p @ v, p @ v.abs())]
-
-
-@pytest.mark.parametrize("variant", [0, 1])   # 0: TMA + wgmma kernel (the network's), 1: mma.sync flash kernel on the same layout
-@pytest.mark.parametrize("B,H", [(1, 1), (2, 4), (3, 12), (64, 16), (5, 16), (7, 6), (33, 12), (128, 16)])
-def test_attention(dev, variant, B, H):
-    lib = _lib.load()
-    D = H * 64
-    g = torch.Generator().manual_seed(B * 100 + H)
-    qkv = torch.randn(B * 256, 3 * D, generator=g).to(dev).bfloat16()
-    ref, pv = attention_ref(qkv.reshape(B, 256, 3, H, 64).permute(0, 1, 3, 2, 4), 64)
-    out = torch.zeros(B * 256, D, device=dev, dtype=torch.bfloat16)
-    rc = lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
-    torch.cuda.synchronize()
-    assert rc == 0, _lib.last_error()
-    assert rel_l2(out.double().cpu(), ref.cpu()) < 5e-3   # P and O are rounded to bf16
-    tk.assert_within(out, ref, tk.bf16_ulp(ref) + 2.0 ** -8 * pv, f"attention B {B} H {H} variant {variant}")
-
-
-@pytest.mark.parametrize("B,H,T,ch,dh", [(2, 4, 1024, 64, 64), (3, 16, 256, 80, 72), (2, 3, 256, 64, 64), (5, 16, 64, 80, 72),
-                                         (7, 16, 16, 80, 72), (1, 2, 128, 80, 72)])
-def test_attention_mma_kernels(dev, B, H, T, ch, dh):
-    """The mma.sync attention kernels of the DiT geometries outside T = 256 / head_dim 64 (head-major qkv rows, heads zero-padded from dh
-    to ch channels) against softmax(q k^T / sqrt(dh)) v in fp64 on the same bf16 operands."""
-    lib = _lib.load()
-    g = torch.Generator().manual_seed(B * 1000 + T + ch)
-    qkv = torch.randn(B, T, H, 3, ch, generator=g)
-    qkv[..., dh:] = 0                                            # the padding channels are zero (zero weight rows)
-    qkv = qkv.reshape(B * T, H * 3 * ch).to(dev).bfloat16()
-    ref, pv = attention_ref(qkv.reshape(B, T, H, 3, ch), dh)
-    out = torch.full((B * T, H * ch), 7.0, device=dev, dtype=torch.bfloat16)
-    rc = lib.lfm_dbg_attention_mma(P(qkv), P(out), B, H, T, ch, dh, None)
-    torch.cuda.synchronize()
-    assert rc == 0, _lib.last_error()
-    assert rel_l2(out.double().cpu(), ref.cpu()) < 5e-3           # P and O are rounded to bf16
-    tk.assert_within(out, ref, tk.bf16_ulp(ref) + 2.0 ** -8 * pv, f"attention_mma B {B} H {H} T {T} ch {ch}")
-    if ch > dh:
-        assert float(out.float().reshape(B * T, H, ch)[..., dh:].abs().max()) == 0.0   # padded output channels are exactly zero
 
 
 # ------------------------------------------------------------------------------------------------ reference fixtures

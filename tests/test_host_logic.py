@@ -48,7 +48,7 @@ def test_every_dit_models_entry_has_the_reference_key_table():
 
 
 def test_padded_head_major_attention_layout_is_equivalent():
-    """The layout contract of the mma.sync attention kernels (csrc/kernels.cuh dit_qkv_*_repack_kernel / dit_proj_weight_pad_kernel,
+    """The layout contract of the mma.sync attention kernels (csrc/kernels.cuh qkv_src_row / dit_proj_weight_pad_kernel,
     restated here): qkv rows re-ordered head-major with head_dim 72 zero-padded to 80, proj columns padded to match.  Attention computed
     in that layout (scale 72^-1/2) followed by the padded projection equals timm's Attention on the original weights."""
     D, H, dh, dhp, T, B = 1152, 16, 72, 80, 16, 2

@@ -117,19 +117,6 @@ def test_kernel_entries_refuse_bad_arguments(lib):
     refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 0.0, None, None, None, 1, 64, None), "eps")
     refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 0, 64, None), "B")
     refused(gn(None, 256, None, 0, None, None, 32, None, None, None, 0, 1, 1e-5, None, None, None, 1, 64, None), "NULL")
-    # lfm_dbg_unet_attention(qkv, out, B, T, C, heads, stream): the shapes no UNet attention kernel covers (see below)
-    att = lib.lfm_dbg_unet_attention
-    refused(att(None, None, 1, 1024, 128, 1, None), "1024 tokens")
-    refused(att(None, None, 1, 64, 384, 1, None), "384 channels")
-    refused(att(None, None, 1, 64, 384, 32, None), "12 channels")
-    refused(att(None, None, 1, 64, 128, 3, None), "heads")
-    refused(att(None, None, 1, 64, 128, 2, None), "NULL")
-    # lfm_dbg_attention_mma(qkv, out, B, H, T, ch, head_dim, stream)
-    mma = lib.lfm_dbg_attention_mma
-    refused(mma(None, None, 1, 1, 64, 96, 0, None), "ch")
-    refused(mma(None, None, 1, 1, 64, 64, 72, None), "head_dim")
-    refused(mma(None, None, 1, 1, 256, 128, 0, None), "T")
-    refused(mma(None, None, 1, 1, 48, 64, 64, None), "T")
     # lfm_dbg_gemm_reversed: lfm_dbg_gemm's checks, under its own name
     rev = lib.lfm_dbg_gemm_reversed
     refused(rev(None, None, None, None, None, 0, 1, 128, 128, 64, 3, 640, None), "block_n")
@@ -170,6 +157,33 @@ def test_kernel_entries_refuse_bad_arguments(lib):
     refused(fl(None, None, None, 2, None, None, None, 256, 384, 16, 4, 2, None), "mod_stride")
     refused(fl(None, None, None, 0, None, None, None, 0, 384, 16, 4, 2, None), "M")
     refused(fl(None, None, None, 0, None, None, None, 256, 384, 16, 4, 2, None), "NULL")
+
+
+def test_attention_entry_refuses_bad_arguments(lib):
+    """lfm_dbg_attention checks its arguments against the attention route table before it touches the device, and names the
+    bad argument: shapes without a route, then bad layouts, head widths, counts and pointers."""
+    from lfm_b200 import _lib
+
+    def refused(rc, word):
+        assert rc != 0
+        assert word in _lib.last_error(), _lib.last_error()
+
+    # lfm_dbg_attention(qkv, out, B, T, heads, ch, head_dim, layout, stream)
+    att = lib.lfm_dbg_attention
+    TIMM, HM = _lib.QKV_TIMM, _lib.QKV_HEAD_MAJOR
+    refused(att(None, None, 1, 1024, 1, 128, 128, HM, None), "1024 tokens")
+    refused(att(None, None, 1, 64, 1, 384, 384, HM, None), "384 channels")
+    refused(att(None, None, 1, 64, 32, 12, 12, HM, None), "12 channels")
+    refused(att(None, None, 1, 1024, 4, 64, 64, TIMM, None), "1024 tokens")   # the timm layout: 256 tokens with 64 channels only
+    refused(att(None, None, 1, 256, 4, 80, 80, TIMM, None), "80 channels")
+    refused(att(None, None, 1, 256, 2, 96, 72, HM, None), "head_dim")         # padded heads on the SIMT kernels
+    refused(att(None, None, 1, 256, 4, 64, 32, TIMM, None), "head_dim")       # ... and on the wgmma kernel
+    refused(att(None, None, 1, 64, 1, 64, 72, HM, None), "head_dim")
+    refused(att(None, None, 1, 64, 1, 64, 0, HM, None), "head_dim")
+    refused(att(None, None, 1, 64, 1, 64, 64, 2, None), "layout")
+    refused(att(None, None, 0, 64, 1, 64, 64, HM, None), "B")
+    refused(att(None, None, 1, 64, 0, 64, 64, HM, None), "heads")
+    refused(att(None, None, 1, 64, 2, 64, 64, HM, None), "NULL")
 
 
 def _unet_desc(cfg):

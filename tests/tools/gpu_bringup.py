@@ -88,17 +88,23 @@ def attn_ref(qkv, B, H):
     return s, o
 
 
+def head_major(qkv, B, H):
+    """The same q, k, v with the rows of each token in head-major order (head * 192 + {q,k,v} * 64 + c)."""
+    return qkv.reshape(B * 256, 3, H, 64).transpose(1, 2).reshape(B * 256, 3 * H * 64).contiguous()
+
+
 def group_attn():
     B, H = 2, 4
     D = H * 64
     g = torch.Generator().manual_seed(3)
     qkv = (torch.randn(B * 256, 3 * D, generator=g)).to(dev).bfloat16()
     s_ref, o_ref = attn_ref(qkv, B, H)
-    for variant in (0, 1):
+    for layout in (_lib.QKV_TIMM, _lib.QKV_HEAD_MAJOR):   # the TMA + wgmma route, the flash route
+        src = qkv if layout == _lib.QKV_TIMM else head_major(qkv, B, H)
         out = torch.zeros(B * 256, D, device=dev, dtype=torch.bfloat16)
-        rc = lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
+        rc = lib.lfm_dbg_attention(P(src), P(out), B, 256, H, 64, 64, layout, None)
         torch.cuda.synchronize()
-        print(f" attention variant {variant} rc={rc} {_lib.last_error() if rc else ''}")
+        print(f" attention layout {layout} rc={rc} {_lib.last_error() if rc else ''}")
         stats("O", out.float(), o_ref)
         # per-q-tile / per-column-block diagnostics
         e = (out.float() - o_ref).abs().reshape(B, 2, 128, H, 64)
@@ -107,18 +113,19 @@ def group_attn():
     D = H * 64
     qkv = (torch.randn(B * 256, 3 * D, generator=g)).to(dev).bfloat16()
     _, o_ref = attn_ref(qkv, B, H)
-    for variant in (0, 1):
+    for layout in (_lib.QKV_TIMM, _lib.QKV_HEAD_MAJOR):
+        src = qkv if layout == _lib.QKV_TIMM else head_major(qkv, B, H)
         out = torch.zeros(B * 256, D, device=dev, dtype=torch.bfloat16)
-        lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
+        lib.lfm_dbg_attention(P(src), P(out), B, 256, H, 64, 64, layout, None)
         torch.cuda.synchronize()
-        stats(f"O full B=64 H=16 variant {variant}", out.float(), o_ref)
+        stats(f"O full B=64 H=16 layout {layout}", out.float(), o_ref)
         t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
         t0.record()
         for _ in range(10):
-            lib.lfm_dbg_attention(P(qkv), P(out), B, H, variant, None, None)
+            lib.lfm_dbg_attention(P(src), P(out), B, 256, H, 64, 64, layout, None)
         t1.record(); torch.cuda.synchronize()
         ms = t0.elapsed_time(t1) / 10
-        print(f"   attention B=64 H=16 variant {variant}: {ms*1e3:.1f} us  ({4*256*256*64*B*H/ms/1e9:.1f} TFLOP/s)")
+        print(f"   attention B=64 H=16 layout {layout}: {ms*1e3:.1f} us  ({4*256*256*64*B*H/ms/1e9:.1f} TFLOP/s)")
 
 
 def group_forward():
