@@ -172,8 +172,17 @@ int lfm_label_condition(const uint8_t* labels, int B, int H, int W, int num_clas
 
 /* nn.Module.load_state_dict (test_flow_latent.py:142): one call per state-dict entry, `key` exactly as in the
  * reference state_dict (SURVEY.md 8(b)); `ptr` may be a host or a device pointer (fp32).  The data is copied
- * (GEMM weights are repacked to bf16).  Unknown key or wrong shape -> error (strict=True behaviour). */
+ * (GEMM weights are repacked to bf16; qkv and fc1 quantised to e4m3 in FP8 mode, see lfm_set_fp8).  Unknown key or wrong shape -> error (strict=True behaviour). */
 int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int dtype, const int64_t* shape, int ndim);
+
+/* FP8 sampling mode of a DiT context (enable != 0; off by default), valid between lfm_create and lfm_set_param of the qkv
+ * and fc1 weights.  Each block's attn.qkv and mlp.fc1 GEMMs then run on e4m3 operands (wgmma k32 e4m3, fp32 accumulation):
+ * ln_modulate writes the LayerNorm + modulate output as e4m3 codes with one fp32 scale per token row (amax / 448), and the
+ * two weights are quantised at upload, from the fp32 source after the qkv re-order and head padding, with one fp32 scale per
+ * output channel; the context keeps only the e4m3 copies.  proj, fc2, attention and everything else stay as they are.  Not a
+ * behaviour of the reference: its results differ from the bf16 path's by the e4m3 rounding of those operands.  Refused after
+ * lfm_finalize, on UNet, EDM and VAE contexts, and once a qkv or fc1 weight has been uploaded in the other mode. */
+int lfm_set_fp8(lfm_ctx* ctx, int enable);
 
 /* After all parameters are set: checks that none is missing (strict), allocates the activation workspace for
  * up to `max_batch` network rows (2x images under CFG) and builds the TMA descriptors. */
@@ -247,6 +256,20 @@ int lfm_dbg_gemm_path(const void* a_bf16, const void* w_bf16, const float* bias,
  * 16-byte aligned, mod_stride a multiple of 4. */
 int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* shift, const float* scale, int mod_stride, int rows_per_sample,
                         int M, int D, int down, void* stream);
+/* The FP8 mode's GEMM (lfm_set_fp8): out = bf16(epi(acc a_scale[m] w_scale[n] + bias[n])), acc = sum_k a[m, k] w[n, k] in fp32
+ * over e4m3 codes a [M, K] and w [N, K] (device), a_scale fp32 [M], w_scale fp32 [N], bias fp32 [N] or NULL, out bf16 [M, N].
+ * epi 0 (bias) or 1 (bias + GELU(tanh)); block_n 0 (the network's pick), 128 or 256.  K % 128 == 0, N % 8 == 0.  Arguments are
+ * checked before the device is touched. */
+int lfm_dbg_gemm_fp8(const void* a_e4m3, const float* a_scale, const void* w_e4m3, const float* w_scale, const float* bias,
+                     void* out_bf16, int M, int N, int K, int epi, int block_n, void* stream);
+/* lfm_dbg_ln_modulate with the FP8 mode's output: v = the modulated fp32 row, y_scale[r] = amax|v| / 448 (1 for an all-zero row),
+ * y[r] = e4m3(v / y_scale[r]) (round to nearest even, saturating).  y e4m3 [M, D], y_scale fp32 [M]; other arguments as
+ * lfm_dbg_ln_modulate. */
+int lfm_dbg_ln_modulate_fp8(const float* x, void* y_e4m3, float* y_scale, const float* shift, const float* scale, int mod_stride,
+                            int rows_per_sample, int M, int D, int down, void* stream);
+/* The FP8 mode's weight quantiser: w fp32 [N, K] (device) -> scales fp32 [N] = amax|w[n, :]| / 448 (1 for an all-zero row) and
+ * codes e4m3 [N, K] = e4m3(w / scales[n]) (round to nearest even, saturating). */
+int lfm_dbg_quantize_rows_fp8(const float* w, void* codes_e4m3, float* scales, int N, int K, void* stream);
 /* The DiT's conditioning for `rows` rows, each stage into a caller-allocated output: tf_out fp32 [rows, 256] timestep features
  * [cos | sin] of t (t_numel 1 or rows), h1_out fp32 [rows, D] = SiLU(w0 tf + b0), c_bf16 bf16 [rows, D] =
  * SiLU(w2 h1 + b2 + table[y[r]]), y NULL = the null row table_rows - 1 for every row.  w0 [D, 256], w2 [D, D], table

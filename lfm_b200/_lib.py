@@ -53,6 +53,7 @@ SYMBOLS = {
     "lfm_encode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "lfm_label_condition": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "lfm_set_param": (C.c_int, [_P, C.c_char_p, _P, C.c_int, C.POINTER(C.c_int64), C.c_int]),
+    "lfm_set_fp8": (C.c_int, [_P, C.c_int]),
     "lfm_finalize": (C.c_int, [_P, C.c_int]),
     "lfm_set_condition": (C.c_int, [_P, _P, C.c_int, C.c_int, _P]),
     "lfm_forward": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_float, _P, _P]),
@@ -70,6 +71,9 @@ SYMBOLS = {
     "lfm_dbg_gemm_path": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, _P]),
     "lfm_dbg_ln_modulate": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_gemm_fp8": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_ln_modulate_fp8": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "lfm_dbg_quantize_rows_fp8": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P]),
     "lfm_dbg_dit_condition": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
     "lfm_dbg_patch_embed": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_final_layer": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

@@ -15,6 +15,7 @@ Differences, all deliberate (SURVEY.md Appendix B):
   * the Karras path works (the reference's CLI raises NameError / TypeError there);
   * ``--device`` exists; nothing is hard-coded to "cuda";
   * ``--synthetic_init SEED`` runs without a checkpoint (seeded non-degenerate weights);
+  * ``--fp8`` (DiT only, off by default) runs the qkv and fc1 GEMMs on e4m3 operands, see lfm_b200.network.DiT;
   * the VAE decode runs natively (lfm_b200.AutoencoderKL: ``--pretrained_autoencoder_ckpt`` = a LOCAL diffusers
     directory, or ``--synthetic_vae SEED``); ``--vae diffusers`` keeps the reference's torch module when that package is
     installed; with neither, latents are saved (``--no_decode``);
@@ -103,6 +104,8 @@ def build_parser():
     p.add_argument("--no_save", action="store_true", help="--compute_fid: do not write the JPEG files")
     p.add_argument("--out_dir", type=str, default=".")
     p.add_argument("--measure_reps", type=int, default=300)
+    p.add_argument("--fp8", action="store_true", default=False,
+                   help="DiT only: run the qkv and fc1 GEMMs on e4m3 operands (H100 FP8 tensor cores); results differ from bf16")
     return p
 
 

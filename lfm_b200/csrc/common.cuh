@@ -4,8 +4,11 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace lfm {
 
@@ -112,6 +115,15 @@ LFM_DEVICE void tma_store_wait() {
 LFM_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
     __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);  // .x = lo (low 16 bits), .y = hi
     return *reinterpret_cast<uint32_t*>(&h);
+}
+// FP8 (e4m3) quantisation of the DiT's FP8 mode: a row of amax |v| gets the scale amax / 448 (448 = the largest finite e4m3), or 1
+// when the row is all zero, so its codes are 0 and nothing divides by zero.  A code is v / scale (IEEE division) rounded to the
+// nearest even e4m3 with saturation - what torch's (v / scale).to(torch.float8_e4m3fn) gives, since |v / scale| <= 448 (+ 1 ulp).
+LFM_DEVICE float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f; }
+LFM_DEVICE uint32_t pack_e4m3x4(float a, float b, float c, float d) {  // a in the low byte
+    const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+    const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
+    return lo | (hi << 16);
 }
 LFM_DEVICE float tanh_fast(float x) {
     float y;

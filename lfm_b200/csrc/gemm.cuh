@@ -15,6 +15,12 @@
 //   EPI_GATE_RESID_F32  x  += gate[b] * (acc + bias)   (fp32 stream) attn.proj / mlp.fc2 + gated residual
 //                                                                    (models/DiT.py:129-130)
 //   EPI_BIAS_F32        out = acc + bias (fp32)                      adaLN_modulation Linears in one GEMM, convolutions
+//
+// FP8 operands (Op = __nv_fp8_e4m3, plain 2-D GEMMs with EPI_BIAS_BF16 / EPI_BIAS_GELU_BF16, the DiT's qkv and fc1 in its FP8
+// mode): A and W hold e4m3 codes with one fp32 scale per A row (GemmEpi::a_scale) and per W row (GemmEpi::w_scale).  A K slab
+// is still one 128-byte swizzle row, now 128 elements, so the stage bytes, the ring and the descriptors are those of bf16; each
+// slab issues four wgmma.m64nBNk32.e4m3 instead of four k16.bf16, and K must be a multiple of 128.  The epilogue starts from
+// acc * a_scale[row] * w_scale[col].
 #pragma once
 #include "common.cuh"
 
@@ -50,6 +56,9 @@ struct GemmEpi {
     // buffer first).  The launch passes the map itself as a kernel parameter; the kernel only tests this pointer.  Plain
     // GEMMs without GroupNorm statistics only; sub-tiles with rows past M keep the register stores.
     const CUtensorMap* out_map = nullptr;
+    // FP8 operands only: the dequantisation scales of the A rows [M] and of the W rows [N].
+    const float* a_scale = nullptr;
+    const float* w_scale = nullptr;
 };
 constexpr int kGnBinReplicas = 16;
 constexpr double kGnFixScale = 268435456.0;  // 2^28: the sum
@@ -80,11 +89,15 @@ struct ConvGeom {
 };
 
 constexpr int kGemmBlockM = 128;
-constexpr int kGemmBlockK = 64;  // 64 bf16 = one 128-byte swizzle row
+constexpr int kGemmBlockK = 64;  // 64 bf16 = one 128-byte swizzle row (128 e4m3: gemm_block_k)
 constexpr int kGemmThreads = 384;
 constexpr int kGemmBoxRows = 128;  // rows of the TMA box of both operand tensor maps
 constexpr int kGemmOutRows = 64;   // rows of an output sub-tile (one consumer warp group) and of the output tensor map's box
 constexpr int kGemmOutBytes = kGemmOutRows * 128;  // one staging buffer: 64 rows of 128 bytes (64 bf16 / 32 fp32 columns)
+
+// K elements of one slab (one 128-byte swizzle row) of operand type Op.
+template <typename Op>
+__host__ __device__ constexpr int gemm_block_k() { return 128 / static_cast<int>(sizeof(Op)); }
 
 template <int BN>
 struct GemmCfg {
@@ -119,36 +132,54 @@ LFM_DEVICE void wgmma_wait() {
 // keeps the compiler from moving accesses of the accumulator registers across the asynchronous wgmma window
 LFM_DEVICE void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
+// The accumulator operands of one wgmma: N / 2 fp32 registers per thread of the warp group (N = 128 or 256).
+#define LFM_WGMMA_ACC64 \
+    "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+    "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define LFM_WGMMA_ACC128 \
+    "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+    "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, " \
+    "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, " \
+    "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, " \
+    "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, " \
+    "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define LFM_WGMMA_ACC64_OPS(d) \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+    "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+    "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+    "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+    "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+    "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define LFM_WGMMA_ACC128_OPS(d) \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+    "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+    "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+    "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+    "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+    "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), \
+    "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+    "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+    "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+    "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+    "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+    "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+    "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+    "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+
 // D[64 x 256] (fp32, registers) += A[64 x 16] (smem) * B[256 x 16]^T (smem), both K-major bf16
 LFM_DEVICE void wgmma_m64n256k16(float* d, uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-        "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {" LFM_WGMMA_ACC128 "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : LFM_WGMMA_ACC128_OPS(d)
         : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
@@ -156,30 +187,43 @@ LFM_DEVICE void wgmma_m64n256k16(float* d, uint64_t desc_a, uint64_t desc_b) {
 LFM_DEVICE void wgmma_m64n128k16(float* d, uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
-        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-        "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {" LFM_WGMMA_ACC64 "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : LFM_WGMMA_ACC64_OPS(d)
         : "l"(desc_a), "l"(desc_b), "r"(1));
 }
 
+// D[64 x 256] += A[64 x 32] * B[256 x 32]^T, both K-major e4m3 (FP8 wgmma takes no transpose operands: K-major only)
+LFM_DEVICE void wgmma_m64n256k32_e4m3(float* d, uint64_t desc_a, uint64_t desc_b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k32.f32.e4m3.e4m3 {" LFM_WGMMA_ACC128 "}, %128, %129, p, 1, 1;\n\t}"
+        : LFM_WGMMA_ACC128_OPS(d)
+        : "l"(desc_a), "l"(desc_b), "r"(1));
+}
 
-template <int BN>
+// D[64 x 128] += A[64 x 32] * B[128 x 32]^T, both K-major e4m3
+LFM_DEVICE void wgmma_m64n128k32_e4m3(float* d, uint64_t desc_a, uint64_t desc_b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {" LFM_WGMMA_ACC64 "}, %64, %65, p, 1, 1;\n\t}"
+        : LFM_WGMMA_ACC64_OPS(d)
+        : "l"(desc_a), "l"(desc_b), "r"(1));
+}
+
+// One 32-byte K step of a 64 x BN tile: k16 for bf16 operands, k32 for e4m3.
+template <int BN, typename Op>
 LFM_DEVICE void wgmma_tile(float* d, uint64_t desc_a, uint64_t desc_b) {
-    if constexpr (BN == 256)
-        wgmma_m64n256k16(d, desc_a, desc_b);
-    else
-        wgmma_m64n128k16(d, desc_a, desc_b);
+    if constexpr (std::is_same_v<Op, __nv_fp8_e4m3>) {
+        if constexpr (BN == 256)
+            wgmma_m64n256k32_e4m3(d, desc_a, desc_b);
+        else
+            wgmma_m64n128k32_e4m3(d, desc_a, desc_b);
+    } else {
+        if constexpr (BN == 256)
+            wgmma_m64n256k16(d, desc_a, desc_b);
+        else
+            wgmma_m64n128k16(d, desc_a, desc_b);
+    }
 }
 
 LFM_DEVICE void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1, int32_t c2, int32_t c3) {
@@ -404,7 +448,7 @@ LFM_DEVICE void epilogue_tma(const float* acc, const GemmEpi& ep, const CUtensor
 // Work items: (tile, k-slice).  ksplit > 1 (split-K, for GEMMs with far fewer tiles than SMs): every slice stores its fp32
 // partial tile, without bias, into its own slab of ep.out (row offset slice * split_row_pitch); a separate kernel adds the
 // slabs in a fixed order.
-template <int BN, int EPI>
+template <int BN, int EPI, typename Op = __nv_bfloat16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the 4-D NHWC activation of a convolution), box 128 rows
                 const __grid_constant__ CUtensorMap tmap_b,  // W [N, K], box {64, 128}
@@ -412,6 +456,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 int M, int N, int K, GemmEpi ep, ConvGeom cg, int ksplit, int split_row_pitch) {
     using Cfg = GemmCfg<BN>;
     constexpr int kStages = Cfg::kStages;
+    constexpr bool kFp8 = std::is_same_v<Op, __nv_fp8_e4m3>;
+    constexpr int kBlockK = gemm_block_k<Op>();
+    static_assert(!kFp8 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU_BF16, "FP8 operands: the bf16-output epilogues only");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
@@ -428,7 +475,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
     const int n_blocks = (N + BN - 1) / BN;
     const int m_blocks = (M + kGemmBlockM - 1) / kGemmBlockM;
     const int num_items = m_blocks * n_blocks * ksplit;
-    const int num_kb = K / kGemmBlockK;
+    const int num_kb = K / kBlockK;
     const int kb_per = (num_kb + ksplit - 1) / ksplit;
     auto decode = [&](int item, int& m_blk, int& n_blk, int& ks) {
         const int tile = item / ksplit;
@@ -483,7 +530,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                     mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
                     uint8_t* sa = smem_a + stage * Cfg::kABytes;
                     if (cg.taps == 0) {
-                        tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kGemmBlockK, row_a);
+                        tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kBlockK, row_a);
                     } else {
                         const int r = tap / 3, sx = tap - 3 * r;
                         tma_load_4d(sa, &tmap_a, &full_bar[stage], cb * 64, cg.stride * w0 + sx - cg.pad, cg.stride * h0 + r - cg.pad, img0);
@@ -494,7 +541,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                     }
 #pragma unroll
                     for (int h = 0; h < BN / kGemmBoxRows; ++h)
-                        tma_load_2d(smem_b + stage * Cfg::kBBytes + h * kGemmBoxRows * 128, &tmap_b, &full_bar[stage], kb * kGemmBlockK,
+                        tma_load_2d(smem_b + stage * Cfg::kBBytes + h * kGemmBoxRows * 128, &tmap_b, &full_bar[stage], kb * kBlockK,
                                     row_b + h * kGemmBoxRows);
                     if (++stage == kStages) {
                         stage = 0;
@@ -538,7 +585,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
                 const uint64_t da = make_wgmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + cw * 64 * 128));
                 const uint64_t db = make_wgmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
 #pragma unroll
-                for (int k = 0; k < kGemmBlockK / 16; ++k) wgmma_tile<BN>(acc, da + 2 * k, db + 2 * k);  // +32 B per K step of 16
+                for (int k = 0; k < 4; ++k) wgmma_tile<BN, Op>(acc, da + 2 * k, db + 2 * k);  // +32 B per K step (16 bf16 / 32 e4m3)
                 wgmma_commit();
                 wgmma_wait<1>();  // the previous slab's MMAs are complete: its slot can be refilled
 #pragma unroll
@@ -554,6 +601,21 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a,  // A [M, K] (or the
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) fence_operand(acc[j]);
             if (kb1 > kb0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            if constexpr (kFp8) {  // dequantise: acc[4 i + {0, 1}] is row r0, acc[4 i + {2, 3}] row r0 + 8 (layout below)
+                const int r0 = m_blk * kGemmBlockM + cw * 64 + warp_in * 16 + (lane >> 2);
+                const float sa0 = __ldg(ep.a_scale + min(r0, M - 1)), sa1 = __ldg(ep.a_scale + min(r0 + 8, M - 1));
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int col = n_blk * BN + 8 * i + 2 * (lane & 3);
+                    if (col < N) {  // N is even
+                        const float sw0 = __ldg(ep.w_scale + col), sw1 = __ldg(ep.w_scale + col + 1);
+                        acc[4 * i] = acc[4 * i] * sa0 * sw0;
+                        acc[4 * i + 1] = acc[4 * i + 1] * sa0 * sw1;
+                        acc[4 * i + 2] = acc[4 * i + 2] * sa1 * sw0;
+                        acc[4 * i + 3] = acc[4 * i + 3] * sa1 * sw1;
+                    }
+                }
+            }
             if (tma_epi) {
                 epilogue_tma<BN, EPI>(acc, ep, &tmap_c, sc, xb, obuf, xphase, grow, n_blk * BN, N, 1 + cw);
                 continue;

@@ -138,6 +138,8 @@ patch_embed_kernel(const float* __restrict__ x, int x_rows, const float* __restr
 // Tiles are dealt round-robin, so the whole grid sweeps M upwards (down = 0) or downwards (down = 1) in time: a sweep that
 // starts where the producer of x finished finds those rows still in L2.
 // rows_per_sample must be a multiple of 16 (launch_ln checks it), so a tile never straddles two samples.
+// OutT = __nv_fp8_e4m3 (the DiT's FP8 mode): the modulated row stays in registers, one more warp reduction takes its amax, and
+// the row is written as e4m3 codes y = v / ys[row] with ys[row] = e4m3_row_scale(amax) (the A operand of the FP8 GEMM).
 constexpr int kLnRows = 16;
 __host__ __device__ constexpr int ln_stages(int NV) { return NV > 8 ? 2 : 3; }  // 3 x 72 KB at D = 1024
 // dynamic shared memory of ln_modulate_kernel<NV>: per stage kLnRows rows of x, then the shift and scale vectors
@@ -150,10 +152,11 @@ LFM_DEVICE void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, u
                  : "memory");
 }
 
-template <int NV>  // NV = D / 128 float4 per lane
+template <int NV, typename OutT = __nv_bfloat16>  // NV = D / 128 float4 per lane
 __global__ void __launch_bounds__(kLnRows * 32, 1)
-ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, const float* __restrict__ shift,
-                   const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int down) {
+ln_modulate_kernel(const float* __restrict__ x, OutT* __restrict__ y, const float* __restrict__ shift,
+                   const float* __restrict__ scale, int mod_stride, int rows_per_sample, int M, int down,
+                   float* __restrict__ ys /* FP8 only: [M] row scales */) {
     constexpr int D = NV * 128;
     constexpr int kLnStages = ln_stages(NV);
     constexpr uint32_t kStageBytes = (kLnRows + 2) * D * 4;
@@ -211,16 +214,36 @@ ln_modulate_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, c
                 ss += (a * a + b * b) + (c * c + d * d);
             }
             const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(D) + 1e-6f);
-            uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
             const float4* shs = reinterpret_cast<const float4*>(ln_smem + stage * kStageBytes + kLnRows * D * 4);
+            if constexpr (std::is_same_v<OutT, __nv_fp8_e4m3>) {
+                float amax = 0.f;
 #pragma unroll
-            for (int m = 0; m < NV; ++m) {
-                const float4 sh = shs[m * 32 + lane], sc = shs[D / 4 + m * 32 + lane];
-                const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
-                const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
-                const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
-                const float d = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
-                yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
+                for (int m = 0; m < NV; ++m) {
+                    const float4 sh = shs[m * 32 + lane], sc = shs[D / 4 + m * 32 + lane];
+                    v[m].x = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
+                    v[m].y = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
+                    v[m].z = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
+                    v[m].w = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
+                    amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[m].x), fabsf(v[m].y)), fmaxf(fabsf(v[m].z), fabsf(v[m].w))));
+                }
+                const float s_row = e4m3_row_scale(warp_max(amax));
+                uint32_t* yp = reinterpret_cast<uint32_t*>(y + static_cast<size_t>(row) * D);
+#pragma unroll
+                for (int m = 0; m < NV; ++m)
+                    yp[m * 32 + lane] = pack_e4m3x4(__fdiv_rn(v[m].x, s_row), __fdiv_rn(v[m].y, s_row), __fdiv_rn(v[m].z, s_row),
+                                                    __fdiv_rn(v[m].w, s_row));
+                if (lane == 0) ys[row] = s_row;
+            } else {
+                uint2* yp = reinterpret_cast<uint2*>(y + static_cast<size_t>(row) * D);
+#pragma unroll
+                for (int m = 0; m < NV; ++m) {
+                    const float4 sh = shs[m * 32 + lane], sc = shs[D / 4 + m * 32 + lane];
+                    const float a = fmaf((v[m].x - mean) * rstd, 1.f + sc.x, sh.x);
+                    const float b = fmaf((v[m].y - mean) * rstd, 1.f + sc.y, sh.y);
+                    const float c = fmaf((v[m].z - mean) * rstd, 1.f + sc.z, sh.z);
+                    const float d = fmaf((v[m].w - mean) * rstd, 1.f + sc.w, sh.w);
+                    yp[m * 32 + lane] = make_uint2(pack_bf16x2(a, b), pack_bf16x2(c, d));
+                }
             }
         }
         __syncthreads();  // every warp has consumed this stage
@@ -709,14 +732,29 @@ LFM_DEVICE int qkv_src_row(int r, int heads, int dh, int dhp, int src, int dst) 
     }
     return src == QKV_EDM ? h * 3 * dh + c * 3 + which : which * heads * dh + h * dh + c;
 }
-// weight [3 C, K] fp32 -> [3 heads dhp, K] bf16
-__global__ void qkv_weight_reorder_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int K, int heads, int dh, int dhp,
+// weight [3 C, K] fp32 -> [3 heads dhp, K] bf16, or fp32 (the source of the FP8 mode's quantisation)
+template <typename OutT>
+__global__ void qkv_weight_reorder_kernel(const float* __restrict__ w, OutT* __restrict__ out, int K, int heads, int dh, int dhp,
                                           int src, int dst) {
     const size_t n = static_cast<size_t>(3) * heads * dhp * K;
     const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int r = qkv_src_row(static_cast<int>(i / K), heads, dh, dhp, src, dst);
-    out[i] = r >= 0 ? __float2bfloat16(w[static_cast<size_t>(r) * K + i % K]) : __float2bfloat16(0.f);
+    out[i] = static_cast<OutT>(r >= 0 ? w[static_cast<size_t>(r) * K + i % K] : 0.f);
+}
+// Per-row e4m3 quantisation of an fp32 weight [N, K] (the FP8 mode's qkv and fc1): scales[n] = e4m3_row_scale(amax |w[n, :]|),
+// codes[n, k] = e4m3(w[n, k] / scales[n]).  One warp per row; zero rows (DiT-XL's padded head channels) get scale 1 and codes 0.
+__global__ void quantize_rows_e4m3_kernel(const float* __restrict__ w, __nv_fp8_e4m3* __restrict__ codes, float* __restrict__ scales,
+                                          int N, int K) {
+    const int row = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (row >= N) return;
+    const float* wr = w + static_cast<size_t>(row) * K;
+    float amax = 0.f;
+    for (int k = lane; k < K; k += 32) amax = fmaxf(amax, fabsf(wr[k]));
+    const float s = e4m3_row_scale(warp_max(amax));
+    uint8_t* cr = reinterpret_cast<uint8_t*>(codes) + static_cast<size_t>(row) * K;
+    for (int k = lane; k < K; k += 32) cr[k] = __nv_cvt_float_to_fp8(__fdiv_rn(wr[k], s), __NV_SATFINITE, __NV_E4M3);
+    if (lane == 0) scales[row] = s;
 }
 // bias [3 C] -> [3 heads dhp], fp32
 __global__ void qkv_bias_reorder_kernel(const float* __restrict__ b, float* __restrict__ out, int heads, int dh, int dhp, int src, int dst) {

@@ -75,6 +75,18 @@ static bool make_tmap_bf16_ld(CUtensorMap* m, const void* base, uint64_t rows, u
 static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     return make_tmap_bf16_ld(m, base, rows, cols, cols, box_rows);
 }
+// Row-major e4m3 matrix [rows, cols] (the FP8 GEMM operands): box = 128 columns (one 128-byte swizzle row) x box_rows rows.
+static bool make_tmap_e4m3(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+    EncodeTiledFn fn = get_encode_fn();
+    if (fn == nullptr) return false;
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {cols};
+    cuuint32_t box[2] = {128, box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
 // GEMM output [rows, cols] (bf16, or fp32 when f32) with a row pitch of ld elements, for the TMA-store epilogue (GemmEpi::out_map):
 // box = 128 bytes x kGemmOutRows rows in the 128-byte swizzle of the staging buffers.  False when the map cannot exist (base or
 // pitch not a multiple of 16 bytes): such outputs keep the register stores.
@@ -139,11 +151,11 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, unsigned block, s
 }
 // ONLY for kernels that execute pdl_wait() before their first global-memory access.
 
-template <int BN, int EPI>
+template <int BN, int EPI, typename Op>
 static cudaError_t launch_gemm_inst(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K,
                                     const GemmEpi& ep, const ConvGeom& cg, int ksplit, int split_row_pitch) {
     static DevOnce once;
-    auto kern = gemm_bf16_wgmma<BN, EPI>;
+    auto kern = gemm_bf16_wgmma<BN, EPI, Op>;
     if (cudaError_t e = smem_opt_in(once, kern, GemmCfg<BN>::kSmemBytes)) return e;
     const int items = ((M + kGemmBlockM - 1) / kGemmBlockM) * ((N + BN - 1) / BN) * ksplit;
     const int grid = items < g_num_sms ? items : g_num_sms;
@@ -161,6 +173,9 @@ static int pick_block_n(int M, int N) {
 // A and W are tensor maps with a box of {64, kGemmBoxRows} (make_tmap_bf16 / make_tmap_act4d); block_n = 128 or 256
 // (0: pick_block_n).  The batched GEMMs of ConvGeom need block_n 256 when N is a multiple of 256 (W rows of one group).
 // Only plain 2-D GEMMs (no taps, no batching, no split-K) without GroupNorm statistics store through ep.out_map.
+// Op = __nv_fp8_e4m3: e4m3 operands (make_tmap_e4m3 maps, ep.a_scale / ep.w_scale set, K % 128 == 0), plain 2-D GEMMs with a
+// bf16 epilogue only.
+template <typename Op = __nv_bfloat16>
 static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int epi,
                                int block_n, const GemmEpi& ep, const ConvGeom& cg = ConvGeom{0, 0, 0, 0, 1}, int ksplit = 1,
                                int split_row_pitch = 0) {
@@ -168,42 +183,57 @@ static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUte
     GemmEpi e = ep;
     if (cg.taps != 0 || cg.batch_m != 0 || ksplit != 1 || ep.gn_bins != nullptr) e.out_map = nullptr;
 #define LFM_GEMM_CASE(BN, E) \
-    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E>(s, ta, tb, M, N, K, e, cg, ksplit, split_row_pitch);
-    LFM_GEMM_CASE(256, EPI_BIAS_BF16)
-    LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
-    LFM_GEMM_CASE(256, EPI_GATE_RESID_F32)
-    LFM_GEMM_CASE(256, EPI_BIAS_F32)
-    LFM_GEMM_CASE(128, EPI_BIAS_BF16)
-    LFM_GEMM_CASE(128, EPI_BIAS_GELU_BF16)
-    LFM_GEMM_CASE(128, EPI_GATE_RESID_F32)
-    LFM_GEMM_CASE(128, EPI_BIAS_F32)
+    if (block_n == BN && epi == E) return launch_gemm_inst<BN, E, Op>(s, ta, tb, M, N, K, e, cg, ksplit, split_row_pitch);
+    if constexpr (std::is_same_v<Op, __nv_fp8_e4m3>) {
+        if (cg.taps != 0 || cg.batch_m != 0 || ksplit != 1 || ep.gn_bins != nullptr || K % 128 != 0) return cudaErrorInvalidValue;
+        LFM_GEMM_CASE(256, EPI_BIAS_BF16)
+        LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
+        LFM_GEMM_CASE(128, EPI_BIAS_BF16)
+        LFM_GEMM_CASE(128, EPI_BIAS_GELU_BF16)
+    } else {
+        LFM_GEMM_CASE(256, EPI_BIAS_BF16)
+        LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
+        LFM_GEMM_CASE(256, EPI_GATE_RESID_F32)
+        LFM_GEMM_CASE(256, EPI_BIAS_F32)
+        LFM_GEMM_CASE(128, EPI_BIAS_BF16)
+        LFM_GEMM_CASE(128, EPI_BIAS_GELU_BF16)
+        LFM_GEMM_CASE(128, EPI_GATE_RESID_F32)
+        LFM_GEMM_CASE(128, EPI_BIAS_F32)
+    }
 #undef LFM_GEMM_CASE
     return cudaErrorInvalidValue;
 }
 
-template <int NV>
-static cudaError_t launch_ln_inst(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
-                                  int mod_stride, int rows_per_sample, int M, int down) {
+template <int NV, typename OutT>
+static cudaError_t launch_ln_inst(cudaStream_t s, const float* x, OutT* y, const float* shift, const float* scale, int mod_stride,
+                                  int rows_per_sample, int M, int down, float* ys) {
     static DevOnce once;
-    auto kern = ln_modulate_kernel<NV>;
+    auto kern = ln_modulate_kernel<NV, OutT>;
     if (cudaError_t e = smem_opt_in(once, kern, ln_smem_bytes(NV))) return e;
     const int tiles = (M + kLnRows - 1) / kLnRows;
     const int grid = tiles < g_num_sms ? tiles : g_num_sms;
-    return launch_k(kern, dim3(grid), kLnRows * 32, ln_smem_bytes(NV), s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+    return launch_k(kern, dim3(grid), kLnRows * 32, ln_smem_bytes(NV), s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
 }
 // down = 0 / 1: the grid sweeps the rows upwards / downwards (ln_modulate_kernel).  A 16-row tile must not straddle two
-// samples: rows_per_sample is a multiple of 16 (the DiT token counts are 16, 64, 256 and 1024).
-static cudaError_t launch_ln(cudaStream_t s, const float* x, __nv_bfloat16* y, const float* shift, const float* scale,
-                             int mod_stride, int rows_per_sample, int M, int D, int down) {
+// samples: rows_per_sample is a multiple of 16 (the DiT token counts are 16, 64, 256 and 1024).  OutT = __nv_fp8_e4m3: e4m3 codes
+// and their row scales ys [M].
+template <typename OutT = __nv_bfloat16>
+static cudaError_t launch_ln(cudaStream_t s, const float* x, OutT* y, const float* shift, const float* scale, int mod_stride,
+                             int rows_per_sample, int M, int D, int down, float* ys = nullptr) {
     if (rows_per_sample % kLnRows != 0) return cudaErrorInvalidValue;
     switch (D / 128) {
-        case 2: return launch_ln_inst<2>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
-        case 3: return launch_ln_inst<3>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
-        case 6: return launch_ln_inst<6>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
-        case 8: return launch_ln_inst<8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
-        case 9: return launch_ln_inst<9>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down);
+        case 2: return launch_ln_inst<2>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
+        case 3: return launch_ln_inst<3>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
+        case 6: return launch_ln_inst<6>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
+        case 8: return launch_ln_inst<8>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
+        case 9: return launch_ln_inst<9>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
         default: return cudaErrorInvalidValue;
     }
+}
+
+// lfm_set_param's per-row e4m3 quantisation (quantize_rows_e4m3_kernel) of an fp32 weight [N, K] on the device.
+static void launch_quantize_rows_e4m3(cudaStream_t s, const float* w, __nv_fp8_e4m3* codes, float* scales, int N, int K) {
+    quantize_rows_e4m3_kernel<<<(N + 7) / 8, 256, 0, s>>>(w, codes, scales, N, K);
 }
 
 static inline unsigned blocks_for(size_t n, int threads = 256) { return static_cast<unsigned>((n + threads - 1) / threads); }
@@ -223,6 +253,8 @@ enum class Xform {
     QKV_B,            //   source order, destination order}
     RESAMPLE_FILTER,  // the constant resample_filter of EDM.py:96-98: validated, not stored
     DIT_PROJ_PAD,     // DiT proj weight with zero columns for the padded head channels (aux = {head dim, its stored width})
+    QKV_W_E4M3,       // FP8 mode: the QKV_W re-order into fp32 (staging), then E4M3_ROWS of the result
+    E4M3_ROWS,        // FP8 mode: e4m3 codes with one fp32 scale per row (ParamSlot::row_scale), from the fp32 source
 };
 
 struct ParamSlot {
@@ -231,6 +263,7 @@ struct ParamSlot {
     size_t numel = 0;
     Xform xform = Xform::F32;
     std::array<int, 4> aux{};
+    float* row_scale = nullptr;  // QKV_W_E4M3 / E4M3_ROWS: [rows of dst]
     bool set = false;
 };
 
@@ -239,9 +272,11 @@ struct ParamSlot {
 enum class NetKind { DIT, ADM, EDM, VAE, VAE_ENC };
 
 struct BlockW {
-    __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;
+    __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;  // w_qkv, w_fc1: NULL in FP8 mode
     float *b_qkv, *b_proj, *b_fc1, *b_fc2;
-    CUtensorMap tm_qkv, tm_proj, tm_fc1, tm_fc2;
+    __nv_fp8_e4m3 *q_qkv = nullptr, *q_fc1 = nullptr;  // FP8 mode: the e4m3 codes of qkv and fc1 ...
+    float *s_qkv = nullptr, *s_fc1 = nullptr;          // ... and their per-row scales
+    CUtensorMap tm_qkv, tm_proj, tm_fc1, tm_fc2;       // tm_qkv, tm_fc1: over the codes in FP8 mode
 };
 
 struct UNetState;
@@ -256,6 +291,7 @@ struct lfm_ctx {
     int in_chw = 0, out_chw = 0;  // floats of one image of the network input / of the solver state and the velocity
     int dh = 64, dhp = 64, Dq = 0;  // head_dim, its stored (zero-padded) width and the width H * dhp of the attention tensors
     int max_rows = 0;
+    bool fp8 = false;  // lfm_set_fp8: qkv and fc1 on e4m3 operands
     bool finalized = false;
     std::string err;
     int64_t launches = 0;
@@ -275,7 +311,9 @@ struct lfm_ctx {
     // workspace
     float *x_tok = nullptr, *mod = nullptr, *tfreq = nullptr, *h1 = nullptr, *v_net = nullptr;
     __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
-    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
+    __nv_fp8_e4m3* xn8 = nullptr;  // FP8 mode: ln_modulate's output as e4m3 codes (instead of xn) ...
+    float* xn_scale = nullptr;     // ... and its row scales
+    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;  // tm_xn: over xn8 in FP8 mode
     CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok, tmo_mod;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
     AttnOp attn_op;  // qkv -> attn of every block
 
@@ -345,6 +383,15 @@ static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::
     return 0;
 }
 
+// Releases one allocation of ctx->allocs (a parameter storage replaced before lfm_finalize).
+static int dev_free(lfm_ctx* ctx, void* p) {
+    if (p == nullptr) return 0;
+    auto it = std::find(ctx->allocs.begin(), ctx->allocs.end(), p);
+    if (it != ctx->allocs.end()) ctx->allocs.erase(it);
+    CUDA_OK(cudaFree(p));
+    return 0;
+}
+
 // Makes the context's device current and gives the launch helpers its SM count: the first step of every entry that uses the device.
 static int bind(lfm_ctx* ctx) {
     CUDA_OK(cudaSetDevice(ctx->device));
@@ -392,6 +439,31 @@ static int finish_create(lfm_ctx* ctx, int rc, lfm_ctx** out) {
     return 0;
 }
 
+// Storage and keys of block i's qkv and fc1 weights, the GEMMs whose A operand ln_modulate writes: bf16, or in FP8 mode (ctx->fp8)
+// e4m3 codes with one fp32 scale per output channel, quantised from the fp32 source after the qkv re-order and head padding.
+static int dit_register_ln_gemm_weights(lfm_ctx* ctx, int i) {
+    BlockW& b = ctx->blk[i];
+    const std::string p = "blocks." + std::to_string(i) + ".";
+    const int D = ctx->D, Dq = ctx->Dq, Hd = ctx->Hd;
+    const int layout = network_qkv_layout(ctx->T, ctx->dhp);
+    if (ctx->fp8) {
+        if (dev_alloc(ctx, &b.q_qkv, (size_t)3 * Dq * D) || dev_alloc(ctx, &b.s_qkv, 3 * Dq) || dev_alloc(ctx, &b.q_fc1, (size_t)Hd * D) ||
+            dev_alloc(ctx, &b.s_fc1, Hd))
+            return 1;
+        add_param(ctx, p + "attn.qkv.weight", b.q_qkv, {3 * D, D}, Xform::QKV_W_E4M3, {ctx->dh, ctx->dhp, QKV_TIMM, layout});
+        ctx->params[p + "attn.qkv.weight"].row_scale = b.s_qkv;
+        add_param(ctx, p + "mlp.fc1.weight", b.q_fc1, {Hd, D}, Xform::E4M3_ROWS);
+        ctx->params[p + "mlp.fc1.weight"].row_scale = b.s_fc1;
+        return 0;
+    }
+    if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
+    if (layout == QKV_HEAD_MAJOR)
+        add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::QKV_W, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
+    else
+        add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::BF16);
+    return alloc_param(ctx, p + "mlp.fc1.weight", &b.w_fc1, {Hd, D}, Xform::BF16);
+}
+
 // DiT parameter storage and state-dict keys.
 static int dit_register(lfm_ctx* ctx) {
     const lfm_model_desc& d = ctx->d;
@@ -419,22 +491,18 @@ static int dit_register(lfm_ctx* ctx) {
         BlockW& b = ctx->blk[i];
         const std::string p = "blocks." + std::to_string(i) + ".";
         // qkv and proj are stored with the padded head width dhp (Dq = H * dhp columns of attention output)
-        if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
+        if (dit_register_ln_gemm_weights(ctx, i)) return 1;
         if (dev_alloc(ctx, &b.b_qkv, 3 * Dq)) return 1;
         if (dev_alloc(ctx, &b.w_proj, (size_t)D * Dq)) return 1;
-        if (network_qkv_layout(T, ctx->dhp) == QKV_HEAD_MAJOR) {
-            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::QKV_W, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
+        if (network_qkv_layout(T, ctx->dhp) == QKV_HEAD_MAJOR)
             add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, Xform::QKV_B, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
-        } else {
-            add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::BF16);
+        else
             add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D});
-        }
         if (ctx->dhp != ctx->dh)
             add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::DIT_PROJ_PAD, {ctx->dh, ctx->dhp});
         else
             add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::BF16);
         if (alloc_param(ctx, p + "attn.proj.bias", &b.b_proj, {D}) ||
-            alloc_param(ctx, p + "mlp.fc1.weight", &b.w_fc1, {Hd, D}, Xform::BF16) ||
             alloc_param(ctx, p + "mlp.fc1.bias", &b.b_fc1, {Hd}) ||
             alloc_param(ctx, p + "mlp.fc2.weight", &b.w_fc2, {D, Hd}, Xform::BF16) ||
             alloc_param(ctx, p + "mlp.fc2.bias", &b.b_fc2, {D}))
@@ -487,6 +555,35 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     return finish_create(ctx, dit_register(ctx), out);
 }
 
+extern "C" int lfm_set_fp8(lfm_ctx* ctx, int enable) {
+    if (ctx == nullptr) return fail(ctx, "lfm_set_fp8: null ctx");
+    if (ctx->net != NetKind::DIT)
+        return fail(ctx, "lfm_set_fp8: FP8 mode exists for the DiT only; this is a %s context",
+                    ctx->net == NetKind::ADM ? "UNet" : ctx->net == NetKind::EDM ? "EDM" : "VAE");
+    if (ctx->finalized) return fail(ctx, "lfm_set_fp8: the context is finalized; call it between lfm_create and lfm_finalize");
+    const bool on = enable != 0;
+    if (on == ctx->fp8) return 0;
+    for (int i = 0; i < ctx->L; ++i)
+        for (const char* w : {"attn.qkv.weight", "mlp.fc1.weight"}) {
+            const std::string key = "blocks." + std::to_string(i) + "." + w;
+            if (ctx->params[key].set)
+                return fail(ctx, "lfm_set_fp8: %s was uploaded in the other mode; call lfm_set_fp8 before lfm_set_param", key.c_str());
+        }
+    if (bind(ctx)) return 1;
+    ctx->fp8 = on;
+    for (int i = 0; i < ctx->L; ++i) {
+        BlockW& b = ctx->blk[i];
+        if (dev_free(ctx, b.w_qkv) || dev_free(ctx, b.w_fc1) || dev_free(ctx, b.q_qkv) || dev_free(ctx, b.s_qkv) ||
+            dev_free(ctx, b.q_fc1) || dev_free(ctx, b.s_fc1))
+            return 1;
+        b.w_qkv = b.w_fc1 = nullptr;
+        b.q_qkv = b.q_fc1 = nullptr;
+        b.s_qkv = b.s_fc1 = nullptr;
+        if (dit_register_ln_gemm_weights(ctx, i)) return 1;
+    }
+    return 0;
+}
+
 extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int dtype, const int64_t* shape, int ndim) {
     if (ctx == nullptr || key == nullptr || ptr == nullptr) return fail(ctx, "lfm_set_param: null argument");
     if (dtype != LFM_DTYPE_F32) return fail(ctx, "lfm_set_param(%s): only fp32 sources are accepted", key);
@@ -501,11 +598,16 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
     if (s.xform == Xform::F32) {
         CUDA_OK(cudaMemcpy(s.dst, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
     } else {
-        if (ctx->staging_elems < s.numel) {
+        // QKV_W_E4M3 re-orders into fp32 behind the source: 3 heads dhp rows of K
+        const size_t reordered = s.xform == Xform::QKV_W_E4M3
+                                     ? static_cast<size_t>(3) * (s.shape[0] / 3 / s.aux[0]) * s.aux[1] * (s.numel / s.shape[0])
+                                     : 0;
+        const size_t need = s.numel + reordered;
+        if (ctx->staging_elems < need) {
             if (ctx->staging != nullptr) CUDA_OK(cudaFree(ctx->staging));
             ctx->staging = nullptr;
-            CUDA_OK(cudaMalloc(&ctx->staging, s.numel * sizeof(float)));
-            ctx->staging_elems = s.numel;
+            CUDA_OK(cudaMalloc(&ctx->staging, need * sizeof(float)));
+            ctx->staging_elems = need;
         }
         CUDA_OK(cudaMemcpy(ctx->staging, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
         switch (s.xform) {
@@ -544,6 +646,20 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
                 CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
                 for (float v : h)
                     if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
+                break;
+            }
+            case Xform::QKV_W_E4M3: {
+                const int dh = s.aux[0], dhp = s.aux[1], heads = static_cast<int>(s.shape[0] / 3) / dh;
+                const int K = static_cast<int>(s.numel / s.shape[0]);
+                float* tmp = ctx->staging + s.numel;
+                qkv_weight_reorder_kernel<<<blocks_for(reordered), 256>>>(ctx->staging, tmp, K, heads, dh, dhp, s.aux[2], s.aux[3]);
+                launch_quantize_rows_e4m3(nullptr, tmp, static_cast<__nv_fp8_e4m3*>(s.dst), s.row_scale, 3 * heads * dhp, K);
+                break;
+            }
+            case Xform::E4M3_ROWS: {
+                const int N = static_cast<int>(s.shape[0]);
+                launch_quantize_rows_e4m3(nullptr, ctx->staging, static_cast<__nv_fp8_e4m3*>(s.dst), s.row_scale, N,
+                                          static_cast<int>(s.numel / N));
                 break;
             }
             case Xform::DIT_PROJ_PAD: {
@@ -603,7 +719,11 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     const size_t M = (size_t)R * T;
     const int Rpad = R < 128 ? 128 : R;
     if (dev_alloc(ctx, &ctx->x_tok, M * D)) return 1;
-    if (dev_alloc(ctx, &ctx->xn, M * D)) return 1;
+    if (ctx->fp8) {
+        if (dev_alloc(ctx, &ctx->xn8, M * D) || dev_alloc(ctx, &ctx->xn_scale, M)) return 1;
+    } else if (dev_alloc(ctx, &ctx->xn, M * D)) {
+        return 1;
+    }
     if (dev_alloc(ctx, &ctx->qkv, M * 3 * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->attn, M * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->hmid, M * Hd)) return 1;
@@ -615,7 +735,7 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (alloc_solver_state(ctx, R)) return 1;
 
     bool ok = true;
-    ok &= make_tmap_bf16(&ctx->tm_xn, ctx->xn, M, D, kGemmBoxRows);
+    ok &= ctx->fp8 ? make_tmap_e4m3(&ctx->tm_xn, ctx->xn8, M, D, kGemmBoxRows) : make_tmap_bf16(&ctx->tm_xn, ctx->xn, M, D, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
@@ -626,9 +746,14 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     ok &= make_tmap_out(&ctx->tmo_x_tok, ctx->x_tok, M, D, D, true);
     ok &= make_tmap_out(&ctx->tmo_mod, ctx->mod, R, ctx->Nmod, ctx->Nmod, true);
     for (auto& b : ctx->blk) {
-        ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, kGemmBoxRows);
+        if (ctx->fp8) {
+            ok &= make_tmap_e4m3(&b.tm_qkv, b.q_qkv, 3 * Dq, D, kGemmBoxRows);
+            ok &= make_tmap_e4m3(&b.tm_fc1, b.q_fc1, Hd, D, kGemmBoxRows);
+        } else {
+            ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, kGemmBoxRows);
+            ok &= make_tmap_bf16(&b.tm_fc1, b.w_fc1, Hd, D, kGemmBoxRows);
+        }
         ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, kGemmBoxRows);
-        ok &= make_tmap_bf16(&b.tm_fc1, b.w_fc1, Hd, D, kGemmBoxRows);
         ok &= make_tmap_bf16(&b.tm_fc2, b.w_fc2, D, Hd, kGemmBoxRows);
     }
     if (!ok) return fail(ctx, "lfm_finalize: cuTensorMapEncodeTiled failed");
@@ -731,15 +856,27 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         dir ^= 1;
         return d;
     };
+    // LayerNorm + modulate into xn, and the GEMM that reads it (qkv, fc1): bf16, or e4m3 with row scales in FP8 mode
+    auto ln = [&](const float* shift, const float* scale) {
+        const int d = next_dir();
+        return ctx->fp8 ? launch_ln(s, ctx->x_tok, ctx->xn8, shift, scale, Nmod, T, M, D, d, ctx->xn_scale)
+                        : launch_ln(s, ctx->x_tok, ctx->xn, shift, scale, Nmod, T, M, D, d);
+    };
+    auto ln_gemm = [&](const CUtensorMap& tw, const float* w_scale, int N, int epi, GemmEpi ep) {
+        ep.reverse_m = next_dir();
+        if (!ctx->fp8) return launch_gemm(s, ctx->tm_xn, tw, M, N, D, epi, 0, ep);
+        ep.a_scale = ctx->xn_scale;
+        ep.w_scale = w_scale;
+        return launch_gemm<__nv_fp8_e4m3>(s, ctx->tm_xn, tw, M, N, D, epi, 0, ep);
+    };
     for (int l = 0; l < L; ++l) {
         BlockW& b = ctx->blk[l];
         const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
-        COUNT_LAUNCH(launch_ln(s, ctx->x_tok, ctx->xn, mb, mb + D, Nmod, T, M, D, next_dir()));
+        COUNT_LAUNCH(ln(mb, mb + D));
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
-            ep.reverse_m = next_dir();
             ep.out_map = &ctx->tmo_qkv;
-            COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_qkv, M, 3 * Dq, D, EPI_BIAS_BF16, 0, ep));
+            COUNT_LAUNCH(ln_gemm(b.tm_qkv, b.s_qkv, 3 * Dq, EPI_BIAS_BF16, ep));
         }
         {
             next_dir();  // attention reads each (sample, head) once: the sweep direction only keeps the GEMMs alternating
@@ -751,12 +888,11 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
             ep.out_map = &ctx->tmo_x_tok;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
         }
-        COUNT_LAUNCH(launch_ln(s, ctx->x_tok, ctx->xn, mb + 3 * D, mb + 4 * D, Nmod, T, M, D, next_dir()));
+        COUNT_LAUNCH(ln(mb + 3 * D, mb + 4 * D));
         {
             GemmEpi ep{b.b_fc1, ctx->hmid, Hd, nullptr, 0, T};
-            ep.reverse_m = next_dir();
             ep.out_map = &ctx->tmo_hmid;
-            COUNT_LAUNCH(launch_gemm(s, ctx->tm_xn, b.tm_fc1, M, Hd, D, EPI_BIAS_GELU_BF16, 0, ep));
+            COUNT_LAUNCH(ln_gemm(b.tm_fc1, b.s_fc1, Hd, EPI_BIAS_GELU_BF16, ep));
         }
         {
             GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};  // x += gate_mlp * fc2(...)   (models/DiT.py:130)
@@ -1409,6 +1545,65 @@ extern "C" int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* sh
     return dbg_run([&](lfm_ctx* ctx) {
         COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<__nv_bfloat16*>(y_bf16), shift, scale, mod_stride,
                                rows_per_sample, M, D, down));
+        return 0;
+    });
+}
+
+// The FP8 mode's kernels, through the launch helpers the DiT forward and lfm_set_param use.
+
+extern "C" int lfm_dbg_gemm_fp8(const void* a_e4m3, const float* a_scale, const void* w_e4m3, const float* w_scale, const float* bias,
+                                void* out_bf16, int M, int N, int K, int epi, int block_n, void* stream) {
+    if (M < 1 || N < 8 || N % 8 != 0 || K < 128 || K % 128 != 0)
+        return fail(nullptr, "lfm_dbg_gemm_fp8: M must be >= 1, N a positive multiple of 8 and K of 128 (got M %d, N %d, K %d)", M, N, K);
+    if (epi != EPI_BIAS_BF16 && epi != EPI_BIAS_GELU_BF16)
+        return fail(nullptr, "lfm_dbg_gemm_fp8: epi must be 0 (bias -> bf16) or 1 (bias + GELU -> bf16) (got %d)", epi);
+    if (block_n != 0 && block_n != 128 && block_n != 256)
+        return fail(nullptr, "lfm_dbg_gemm_fp8: block_n must be 0, 128 or 256 (got %d)", block_n);
+    if (a_e4m3 == nullptr || a_scale == nullptr || w_e4m3 == nullptr || w_scale == nullptr || out_bf16 == nullptr)
+        return fail(nullptr, "lfm_dbg_gemm_fp8: a, a_scale, w, w_scale and out must not be NULL (bias may be)");
+    return dbg_run([&](lfm_ctx* ctx) {
+        CUtensorMap ta, tb, tc;
+        if (!make_tmap_e4m3(&ta, a_e4m3, M, K, kGemmBoxRows) || !make_tmap_e4m3(&tb, w_e4m3, N, K, kGemmBoxRows))
+            return fail(ctx, "lfm_dbg_gemm_fp8: tensor map encode failed");
+        GemmEpi ep{bias, out_bf16, N, nullptr, 0, 1};
+        ep.out_map = make_tmap_out(&tc, out_bf16, M, N, N, false) ? &tc : nullptr;
+        ep.a_scale = a_scale;
+        ep.w_scale = w_scale;
+        COUNT_LAUNCH(launch_gemm<__nv_fp8_e4m3>(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
+        return 0;
+    });
+}
+
+extern "C" int lfm_dbg_ln_modulate_fp8(const float* x, void* y_e4m3, float* y_scale, const float* shift, const float* scale, int mod_stride,
+                                       int rows_per_sample, int M, int D, int down, void* stream) {
+    const int nv = D / 128;
+    if (D % 128 != 0 || !(nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9))
+        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: D must be 128 x {2, 3, 6, 8, 9} (got %d)", D);
+    if (rows_per_sample < kLnRows || rows_per_sample % kLnRows != 0)
+        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: rows_per_sample must be a positive multiple of %d (got %d)", kLnRows,
+                    rows_per_sample);
+    if (M < 1) return fail(nullptr, "lfm_dbg_ln_modulate_fp8: M must be >= 1 (got %d)", M);
+    if (mod_stride < 0 || mod_stride % 4 != 0)
+        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
+    if (down != 0 && down != 1) return fail(nullptr, "lfm_dbg_ln_modulate_fp8: down must be 0 or 1 (got %d)", down);
+    if (x == nullptr || y_e4m3 == nullptr || y_scale == nullptr || shift == nullptr || scale == nullptr || !aligned16(x) ||
+        !aligned16(y_e4m3) || !aligned16(shift) || !aligned16(scale))
+        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: x, y, y_scale, shift and scale must not be NULL (x, y, shift and scale "
+                             "16-byte aligned)");
+    return dbg_run([&](lfm_ctx* ctx) {
+        COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<__nv_fp8_e4m3*>(y_e4m3), shift, scale, mod_stride,
+                               rows_per_sample, M, D, down, y_scale));
+        return 0;
+    });
+}
+
+extern "C" int lfm_dbg_quantize_rows_fp8(const float* w, void* codes_e4m3, float* scales, int N, int K, void* stream) {
+    if (N < 1 || K < 1) return fail(nullptr, "lfm_dbg_quantize_rows_fp8: N and K must be >= 1 (got N %d, K %d)", N, K);
+    if (w == nullptr || codes_e4m3 == nullptr || scales == nullptr)
+        return fail(nullptr, "lfm_dbg_quantize_rows_fp8: w, codes and scales must not be NULL");
+    return dbg_run([&](lfm_ctx* ctx) {
+        launch_quantize_rows_e4m3(static_cast<cudaStream_t>(stream), w, static_cast<__nv_fp8_e4m3*>(codes_e4m3), scales, N, K);
+        LAUNCH_OK();
         return 0;
     });
 }

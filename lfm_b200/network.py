@@ -185,10 +185,14 @@ class _NativeNet(nn.Module):
 
 
 class DiT(_NativeNet):
-    """H100-native DiT velocity network with the reference's constructor (models/DiT.py:157-169)."""
+    """H100-native DiT velocity network with the reference's constructor (models/DiT.py:157-169).
+
+    ``fp8=True`` (not a reference option; off by default) runs each block's attn.qkv and mlp.fc1 GEMMs on e4m3 operands:
+    per-token activation scales from the LayerNorm-modulate pass, per-output-channel weight scales taken at upload from the
+    fp32 parameters (include/lfm_b200.h, lfm_set_fp8).  The results then differ from the bf16 path's by that rounding."""
 
     def __init__(self, img_resolution=32, patch_size=2, in_channels=4, hidden_size=1152, depth=28, num_heads=16,
-                 mlp_ratio=4.0, label_dropout=0.1, num_classes=1000, learn_sigma=False, max_batch=None):
+                 mlp_ratio=4.0, label_dropout=0.1, num_classes=1000, learn_sigma=False, max_batch=None, fp8=False):
         super().__init__()
         if learn_sigma:
             raise NotImplementedError("learn_sigma=True is not used by the LFM sampling path")
@@ -199,6 +203,7 @@ class DiT(_NativeNet):
         self.label_dropout = label_dropout
         self.table_rows = num_classes + (1 if label_dropout > 0 else 0)  # models/DiT.py:79-81
         self.max_batch_hint = max_batch
+        self.fp8 = bool(fp8)
 
         self.x_embedder = _Holder()
         self.x_embedder.proj = nn.Conv2d(in_channels, D, kernel_size=patch_size, stride=patch_size, bias=True)
@@ -253,6 +258,12 @@ class DiT(_NativeNet):
                               self.num_heads, self.mlp_hidden, self.table_rows)
         ctx = C.c_void_p()
         _lib.check(lib.lfm_create(C.byref(desc), dev_index, C.byref(ctx)))
+        if self.fp8:
+            rc = lib.lfm_set_fp8(ctx, 1)
+            if rc != 0:
+                msg = _lib.last_error(ctx)
+                lib.lfm_destroy(ctx)
+                raise RuntimeError("liblfm_b200: " + msg)
         return ctx
 
     # -- model(t, x, y)  (reference models/DiT.py:252-272) -----------------------------------------------------
@@ -293,7 +304,12 @@ DiT_models = {
 
 def create_network(config):
     """reference models/__init__.py:6-17: UNetModel (--use_origin_adm), the EDM family (model_type without "DiT":
-    only "adm" = DhariwalUNet is native) or a DiT."""
+    only "adm" = DhariwalUNet is native) or a DiT.  ``config.fp8`` (absent = False) selects the DiT's FP8 mode, which
+    the UNets do not have."""
+    fp8 = bool(getattr(config, "fp8", False))
+    if fp8 and (getattr(config, "use_origin_adm", False) or "DiT" not in config.model_type):
+        raise ValueError("fp8 is implemented for the DiT models only, not for the ADM / EDM UNets "
+                         f"(model_type {config.model_type!r}, use_origin_adm {getattr(config, 'use_origin_adm', False)})")
     if getattr(config, "use_origin_adm", False):
         return get_flow_model(config)
     if "DiT" not in config.model_type:
@@ -304,6 +320,7 @@ def create_network(config):
         in_channels=config.num_in_channels,
         label_dropout=config.label_dropout,
         num_classes=config.num_classes,
+        fp8=fp8,
     )
 
 
