@@ -58,50 +58,49 @@ static EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
+// One tensor map of `rank` dimensions (innermost first; strides in bytes, of dimensions 1 .. rank - 1) in the 128-byte swizzle of
+// every GEMM operand and output staging buffer.
+static bool encode_tmap(CUtensorMap* m, CUtensorMapDataType dtype, cuuint32_t rank, const void* base, const cuuint64_t* dims,
+                        const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* elem_strides) {
+    EncodeTiledFn fn = get_encode_fn();
+    return fn != nullptr && fn(m, dtype, rank, const_cast<void*>(base), dims, strides, box, elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+static const cuuint32_t kUnitStrides[4] = {1, 1, 1, 1};
+
 // Row-major bf16 matrix [rows, cols] with a row pitch of ld elements (ld > cols: a column window of a wider matrix);
 // box = 64 columns (one 128-byte swizzle row) x box_rows rows.
 static bool make_tmap_bf16_ld(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (fn == nullptr) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {64, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
+    const cuuint64_t dims[2] = {cols, rows}, strides[1] = {ld * 2};
+    const cuuint32_t box[2] = {64, box_rows};
+    return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box, kUnitStrides);
 }
 static bool make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
     return make_tmap_bf16_ld(m, base, rows, cols, cols, box_rows);
 }
 // Row-major e4m3 matrix [rows, cols] (the FP8 GEMM operands): box = 128 columns (one 128-byte swizzle row) x box_rows rows.
 static bool make_tmap_e4m3(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (fn == nullptr) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols};
-    cuuint32_t box[2] = {128, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
+    const cuuint64_t dims[2] = {cols, rows}, strides[1] = {cols};
+    const cuuint32_t box[2] = {128, box_rows};
+    return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, strides, box, kUnitStrides);
+}
+// A GEMM operand [rows, cols] of element type Op (bf16 or e4m3, the launch_gemm<Op> operand), box rows kGemmBoxRows.
+template <typename Op>
+static bool make_tmap_operand(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols) {
+    if constexpr (std::is_same_v<Op, __nv_fp8_e4m3>) return make_tmap_e4m3(m, base, rows, cols, kGemmBoxRows);
+    return make_tmap_bf16(m, base, rows, cols, kGemmBoxRows);
 }
 // GEMM output [rows, cols] (bf16, or fp32 when f32) with a row pitch of ld elements, for the TMA-store epilogue (GemmEpi::out_map):
 // box = 128 bytes x kGemmOutRows rows in the 128-byte swizzle of the staging buffers.  False when the map cannot exist (base or
 // pitch not a multiple of 16 bytes): such outputs keep the register stores.
 static bool make_tmap_out(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, bool f32) {
     const uint64_t es = f32 ? 4 : 2;
-    EncodeTiledFn fn = get_encode_fn();
-    if (fn == nullptr || (reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * es) % 16 != 0) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld * es};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / es), static_cast<cuuint32_t>(kGemmOutRows)};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims,
-                    strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
+    if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld * es) % 16 != 0) return false;
+    const cuuint64_t dims[2] = {cols, rows}, strides[1] = {ld * es};
+    const cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / es), static_cast<cuuint32_t>(kGemmOutRows)};
+    return encode_tmap(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box,
+                       kUnitStrides);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -173,8 +172,8 @@ static int pick_block_n(int M, int N) {
 // A and W are tensor maps with a box of {64, kGemmBoxRows} (make_tmap_bf16 / make_tmap_act4d); block_n = 128 or 256
 // (0: pick_block_n).  The batched GEMMs of ConvGeom need block_n 256 when N is a multiple of 256 (W rows of one group).
 // Only plain 2-D GEMMs (no taps, no batching, no split-K) without GroupNorm statistics store through ep.out_map.
-// Op = __nv_fp8_e4m3: e4m3 operands (make_tmap_e4m3 maps, ep.a_scale / ep.w_scale set, K % 128 == 0), plain 2-D GEMMs with a
-// bf16 epilogue only.
+// Op = __nv_fp8_e4m3: e4m3 operands (make_tmap_e4m3 maps, ep.a_scale / ep.w_scale set), plain 2-D GEMMs with a bf16 epilogue
+// only.  K is a multiple of gemm_block_k<Op>(): 64 for bf16, 128 for e4m3.
 template <typename Op = __nv_bfloat16>
 static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUtensorMap& tb, int M, int N, int K, int epi,
                                int block_n, const GemmEpi& ep, const ConvGeom& cg = ConvGeom{0, 0, 0, 0, 1}, int ksplit = 1,
@@ -185,7 +184,8 @@ static cudaError_t launch_gemm(cudaStream_t s, const CUtensorMap& ta, const CUte
 #define LFM_GEMM_CASE(BN, E) \
     if (block_n == BN && epi == E) return launch_gemm_inst<BN, E, Op>(s, ta, tb, M, N, K, e, cg, ksplit, split_row_pitch);
     if constexpr (std::is_same_v<Op, __nv_fp8_e4m3>) {
-        if (cg.taps != 0 || cg.batch_m != 0 || ksplit != 1 || ep.gn_bins != nullptr || K % 128 != 0) return cudaErrorInvalidValue;
+        if (cg.taps != 0 || cg.batch_m != 0 || ksplit != 1 || ep.gn_bins != nullptr || K % gemm_block_k<Op>() != 0)
+            return cudaErrorInvalidValue;
         LFM_GEMM_CASE(256, EPI_BIAS_BF16)
         LFM_GEMM_CASE(256, EPI_BIAS_GELU_BF16)
         LFM_GEMM_CASE(128, EPI_BIAS_BF16)
@@ -214,13 +214,21 @@ static cudaError_t launch_ln_inst(cudaStream_t s, const float* x, OutT* y, const
     const int grid = tiles < g_num_sms ? tiles : g_num_sms;
     return launch_k(kern, dim3(grid), kLnRows * 32, ln_smem_bytes(NV), s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
 }
-// down = 0 / 1: the grid sweeps the rows upwards / downwards (ln_modulate_kernel).  A 16-row tile must not straddle two
-// samples: rows_per_sample is a multiple of 16 (the DiT token counts are 16, 64, 256 and 1024).  OutT = __nv_fp8_e4m3: e4m3 codes
-// and their row scales ys [M].
-template <typename OutT = __nv_bfloat16>
+// The widths ln_modulate_kernel is instantiated for (launch_ln's switch): D = 128 NV with NV in {2, 3, 6, 8, 9}, the hidden sizes
+// 256, 384, 768, 1024 and 1152.
+static bool ln_width_ok(int D) {
+    const int nv = D / 128;
+    return D % 128 == 0 && (nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9);
+}
+// A kLnRows-row tile must not straddle two samples (the DiT token counts are 16, 64, 256 and 1024).
+static bool ln_rows_per_sample_ok(int rows_per_sample) { return rows_per_sample > 0 && rows_per_sample % kLnRows == 0; }
+
+// down = 0 / 1: the grid sweeps the rows upwards / downwards (ln_modulate_kernel).  OutT = __nv_fp8_e4m3: e4m3 codes and their row
+// scales ys [M] (NULL for bf16).
+template <typename OutT>
 static cudaError_t launch_ln(cudaStream_t s, const float* x, OutT* y, const float* shift, const float* scale, int mod_stride,
-                             int rows_per_sample, int M, int D, int down, float* ys = nullptr) {
-    if (rows_per_sample % kLnRows != 0) return cudaErrorInvalidValue;
+                             int rows_per_sample, int M, int D, int down, float* ys) {
+    if (!ln_width_ok(D) || !ln_rows_per_sample_ok(rows_per_sample)) return cudaErrorInvalidValue;
     switch (D / 128) {
         case 2: return launch_ln_inst<2>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
         case 3: return launch_ln_inst<3>(s, x, y, shift, scale, mod_stride, rows_per_sample, M, down, ys);
@@ -230,6 +238,9 @@ static cudaError_t launch_ln(cudaStream_t s, const float* x, OutT* y, const floa
         default: return cudaErrorInvalidValue;
     }
 }
+
+// Patch sizes with a patch-embed and a final-layer kernel (launch_patch_embed, launch_final_layer): 2, and 4 or 8 on the generic ones.
+static bool dit_patch_ok(int p) { return p == 2 || p == 4 || p == 8; }
 
 // lfm_set_param's per-row e4m3 quantisation (quantize_rows_e4m3_kernel) of an fp32 weight [N, K] on the device.
 static void launch_quantize_rows_e4m3(cudaStream_t s, const float* w, __nv_fp8_e4m3* codes, float* scales, int N, int K) {
@@ -243,27 +254,31 @@ static inline unsigned blocks_for(size_t n, int threads = 256) { return static_c
 // ------------------------------------------------------------------------------------------------
 // context
 
-// What lfm_set_param makes of an fp32 source.  Every transform but F32 reads the source from the staging buffer.
-enum class Xform {
-    F32,              // plain fp32 copy
-    BF16,             // cast to bf16
-    CONV_BF16,        // conv weight [Co, Ci, kh, kw] -> bf16 [Co, kh, kw, Ci]
-    TRANSPOSE_F32,    // fp32 [R, rest] -> [rest, R]
-    QKV_W,            // qkv weight (bf16) / bias (fp32) rows re-ordered, qkv_src_row: aux = {head dim, its stored width,
-    QKV_B,            //   source order, destination order}
+// What lfm_set_param makes of an fp32 source: a layout of its elements ...
+enum class Layout {
+    COPY,             // as given
+    CONV,             // conv weight [Co, Ci, kh, kw] -> [Co, kh, kw, Ci]
+    TRANSPOSE,        // [R, rest] -> [rest, R]
+    QKV_W,            // qkv weight / bias rows re-ordered, qkv_src_row: aux = {head dim, its stored width, source order,
+    QKV_B,            //   destination order}
+    PROJ_PAD,         // DiT proj weight with zero columns for the padded head channels (aux = {head dim, its stored width})
     RESAMPLE_FILTER,  // the constant resample_filter of EDM.py:96-98: validated, not stored
-    DIT_PROJ_PAD,     // DiT proj weight with zero columns for the padded head channels (aux = {head dim, its stored width})
-    QKV_W_E4M3,       // FP8 mode: the QKV_W re-order into fp32 (staging), then E4M3_ROWS of the result
-    E4M3_ROWS,        // FP8 mode: e4m3 codes with one fp32 scale per row (ParamSlot::row_scale), from the fp32 source
+};
+// ... stored as one of these types.
+enum class Store {
+    F32,
+    BF16,
+    E4M3_ROWS,  // e4m3 codes with one fp32 scale per row (ParamSlot::row_scale): the FP8 mode's qkv and fc1 weights
 };
 
 struct ParamSlot {
-    void* dst = nullptr;        // device destination (fp32 or bf16)
+    void* dst = nullptr;  // device destination
     std::vector<int64_t> shape;
     size_t numel = 0;
-    Xform xform = Xform::F32;
+    Layout layout = Layout::COPY;
+    Store store = Store::F32;
     std::array<int, 4> aux{};
-    float* row_scale = nullptr;  // QKV_W_E4M3 / E4M3_ROWS: [rows of dst]
+    float* row_scale = nullptr;  // E4M3_ROWS: [rows of dst]
     bool set = false;
 };
 
@@ -272,11 +287,11 @@ struct ParamSlot {
 enum class NetKind { DIT, ADM, EDM, VAE, VAE_ENC };
 
 struct BlockW {
-    __nv_bfloat16 *w_qkv, *w_proj, *w_fc1, *w_fc2;  // w_qkv, w_fc1: NULL in FP8 mode
+    void *w_qkv, *w_fc1;                     // the LayerNorm-fed weights, in the operand type of the mode (with_ln_operand) ...
+    float *s_qkv = nullptr, *s_fc1 = nullptr;  // ... and their per-row scales (NULL for bf16)
+    __nv_bfloat16 *w_proj, *w_fc2;
     float *b_qkv, *b_proj, *b_fc1, *b_fc2;
-    __nv_fp8_e4m3 *q_qkv = nullptr, *q_fc1 = nullptr;  // FP8 mode: the e4m3 codes of qkv and fc1 ...
-    float *s_qkv = nullptr, *s_fc1 = nullptr;          // ... and their per-row scales
-    CUtensorMap tm_qkv, tm_proj, tm_fc1, tm_fc2;       // tm_qkv, tm_fc1: over the codes in FP8 mode
+    CUtensorMap tm_qkv, tm_proj, tm_fc1, tm_fc2;
 };
 
 struct UNetState;
@@ -310,10 +325,10 @@ struct lfm_ctx {
 
     // workspace
     float *x_tok = nullptr, *mod = nullptr, *tfreq = nullptr, *h1 = nullptr, *v_net = nullptr;
-    __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
-    __nv_fp8_e4m3* xn8 = nullptr;  // FP8 mode: ln_modulate's output as e4m3 codes (instead of xn) ...
-    float* xn_scale = nullptr;     // ... and its row scales
-    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;  // tm_xn: over xn8 in FP8 mode
+    void* xn = nullptr;            // ln_modulate's output, in the operand type of the mode (with_ln_operand) ...
+    float* xn_scale = nullptr;     // ... and its row scales (NULL for bf16)
+    __nv_bfloat16 *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
+    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
     CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok, tmo_mod;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
     AttnOp attn_op;  // qkv -> attn of every block
 
@@ -363,23 +378,25 @@ static size_t numel(const std::vector<int64_t>& shape) {
     return n;
 }
 
-static void add_param(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, Xform xform = Xform::F32,
-                      std::array<int, 4> aux = {}) {
+static void add_param(lfm_ctx* ctx, const std::string& key, void* dst, std::vector<int64_t> shape, Layout layout = Layout::COPY,
+                      Store store = Store::F32, std::array<int, 4> aux = {}, float* row_scale = nullptr) {
     ParamSlot s;
     s.dst = dst;
     s.numel = numel(shape);
     s.shape = std::move(shape);
-    s.xform = xform;
+    s.layout = layout;
+    s.store = store;
     s.aux = aux;
+    s.row_scale = row_scale;
     ctx->params[key] = s;
 }
 
 // A parameter whose storage holds exactly its registered shape: allocate numel(shape) elements and register them.
 template <typename Tp>
-static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::vector<int64_t>& shape, Xform xform = Xform::F32,
-                       std::array<int, 4> aux = {}) {
+static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::vector<int64_t>& shape, Layout layout = Layout::COPY,
+                       Store store = Store::F32, std::array<int, 4> aux = {}) {
     if (dev_alloc(ctx, p, numel(shape))) return 1;
-    add_param(ctx, key, *p, shape, xform, aux);
+    add_param(ctx, key, *p, shape, layout, store, aux);
     return 0;
 }
 
@@ -445,23 +462,19 @@ static int dit_register_ln_gemm_weights(lfm_ctx* ctx, int i) {
     BlockW& b = ctx->blk[i];
     const std::string p = "blocks." + std::to_string(i) + ".";
     const int D = ctx->D, Dq = ctx->Dq, Hd = ctx->Hd;
+    const Store store = ctx->fp8 ? Store::E4M3_ROWS : Store::BF16;
+    const size_t es = ctx->fp8 ? 1 : 2;
+    uint8_t *qkv, *fc1;
+    if (dev_alloc(ctx, &qkv, es * 3 * Dq * D) || dev_alloc(ctx, &fc1, es * Hd * D)) return 1;
+    b.w_qkv = qkv;
+    b.w_fc1 = fc1;
+    b.s_qkv = b.s_fc1 = nullptr;
+    if (store == Store::E4M3_ROWS && (dev_alloc(ctx, &b.s_qkv, 3 * Dq) || dev_alloc(ctx, &b.s_fc1, Hd))) return 1;
     const int layout = network_qkv_layout(ctx->T, ctx->dhp);
-    if (ctx->fp8) {
-        if (dev_alloc(ctx, &b.q_qkv, (size_t)3 * Dq * D) || dev_alloc(ctx, &b.s_qkv, 3 * Dq) || dev_alloc(ctx, &b.q_fc1, (size_t)Hd * D) ||
-            dev_alloc(ctx, &b.s_fc1, Hd))
-            return 1;
-        add_param(ctx, p + "attn.qkv.weight", b.q_qkv, {3 * D, D}, Xform::QKV_W_E4M3, {ctx->dh, ctx->dhp, QKV_TIMM, layout});
-        ctx->params[p + "attn.qkv.weight"].row_scale = b.s_qkv;
-        add_param(ctx, p + "mlp.fc1.weight", b.q_fc1, {Hd, D}, Xform::E4M3_ROWS);
-        ctx->params[p + "mlp.fc1.weight"].row_scale = b.s_fc1;
-        return 0;
-    }
-    if (dev_alloc(ctx, &b.w_qkv, (size_t)3 * Dq * D)) return 1;
-    if (layout == QKV_HEAD_MAJOR)
-        add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::QKV_W, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
-    else
-        add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, Xform::BF16);
-    return alloc_param(ctx, p + "mlp.fc1.weight", &b.w_fc1, {Hd, D}, Xform::BF16);
+    add_param(ctx, p + "attn.qkv.weight", b.w_qkv, {3 * D, D}, layout == QKV_HEAD_MAJOR ? Layout::QKV_W : Layout::COPY, store,
+              {ctx->dh, ctx->dhp, QKV_TIMM, layout}, b.s_qkv);
+    add_param(ctx, p + "mlp.fc1.weight", b.w_fc1, {Hd, D}, Layout::COPY, store, {}, b.s_fc1);
+    return 0;
 }
 
 // DiT parameter storage and state-dict keys.
@@ -471,7 +484,7 @@ static int dit_register(lfm_ctx* ctx) {
     const int ps = d.patch_size;
     const int P = ctx->C * ps * ps;  // elements of one patch = out-features of the final linear
     if (alloc_param(ctx, "pos_embed", &ctx->pos, {1, T, D}) ||
-        alloc_param(ctx, "x_embedder.proj.weight", &ctx->pe_w, {D, 4, ps, ps}, Xform::TRANSPOSE_F32) ||  // stored as [P, D]
+        alloc_param(ctx, "x_embedder.proj.weight", &ctx->pe_w, {D, 4, ps, ps}, Layout::TRANSPOSE) ||  // stored as [P, D]
         alloc_param(ctx, "x_embedder.proj.bias", &ctx->pe_b, {D}) ||
         alloc_param(ctx, "t_embedder.mlp.0.weight", &ctx->t_w0, {D, 256}) ||
         alloc_param(ctx, "t_embedder.mlp.0.bias", &ctx->t_b0, {D}) ||
@@ -484,7 +497,7 @@ static int dit_register(lfm_ctx* ctx) {
     // all adaLN modulation layers in one table: block i at rows 6 i D, the final layer's after them
     if (dev_alloc(ctx, &ctx->w_mod, (size_t)ctx->Nmod * D)) return 1;
     if (dev_alloc(ctx, &ctx->b_mod, ctx->Nmod)) return 1;
-    add_param(ctx, "final_layer.adaLN_modulation.1.weight", ctx->w_mod + (size_t)6 * L * D * D, {2 * D, D}, Xform::BF16);
+    add_param(ctx, "final_layer.adaLN_modulation.1.weight", ctx->w_mod + (size_t)6 * L * D * D, {2 * D, D}, Layout::COPY, Store::BF16);
     add_param(ctx, "final_layer.adaLN_modulation.1.bias", ctx->b_mod + (size_t)6 * L * D, {2 * D});
     ctx->blk.resize(L);
     for (int i = 0; i < L; ++i) {
@@ -494,20 +507,17 @@ static int dit_register(lfm_ctx* ctx) {
         if (dit_register_ln_gemm_weights(ctx, i)) return 1;
         if (dev_alloc(ctx, &b.b_qkv, 3 * Dq)) return 1;
         if (dev_alloc(ctx, &b.w_proj, (size_t)D * Dq)) return 1;
-        if (network_qkv_layout(T, ctx->dhp) == QKV_HEAD_MAJOR)
-            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, Xform::QKV_B, {ctx->dh, ctx->dhp, QKV_TIMM, QKV_HEAD_MAJOR});
-        else
-            add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D});
-        if (ctx->dhp != ctx->dh)
-            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::DIT_PROJ_PAD, {ctx->dh, ctx->dhp});
-        else
-            add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, Xform::BF16);
+        const int layout = network_qkv_layout(T, ctx->dhp);
+        add_param(ctx, p + "attn.qkv.bias", b.b_qkv, {3 * D}, layout == QKV_HEAD_MAJOR ? Layout::QKV_B : Layout::COPY, Store::F32,
+                  {ctx->dh, ctx->dhp, QKV_TIMM, layout});
+        add_param(ctx, p + "attn.proj.weight", b.w_proj, {D, D}, ctx->dhp != ctx->dh ? Layout::PROJ_PAD : Layout::COPY, Store::BF16,
+                  {ctx->dh, ctx->dhp});
         if (alloc_param(ctx, p + "attn.proj.bias", &b.b_proj, {D}) ||
             alloc_param(ctx, p + "mlp.fc1.bias", &b.b_fc1, {Hd}) ||
-            alloc_param(ctx, p + "mlp.fc2.weight", &b.w_fc2, {D, Hd}, Xform::BF16) ||
+            alloc_param(ctx, p + "mlp.fc2.weight", &b.w_fc2, {D, Hd}, Layout::COPY, Store::BF16) ||
             alloc_param(ctx, p + "mlp.fc2.bias", &b.b_fc2, {D}))
             return 1;
-        add_param(ctx, p + "adaLN_modulation.1.weight", ctx->w_mod + (size_t)i * 6 * D * D, {6 * D, D}, Xform::BF16);
+        add_param(ctx, p + "adaLN_modulation.1.weight", ctx->w_mod + (size_t)i * 6 * D * D, {6 * D, D}, Layout::COPY, Store::BF16);
         add_param(ctx, p + "adaLN_modulation.1.bias", ctx->b_mod + (size_t)i * 6 * D, {6 * D});
     }
     return 0;
@@ -519,7 +529,7 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     if (desc->arch != LFM_ARCH_DIT) return fail(nullptr, "lfm_create: unsupported arch %d", desc->arch);
     // Geometries (models/DiT.py:355-415; img_resolution = image_size // f): patch 2 / 4 / 8 on latents whose token grid is
     // 4 x 4, 8 x 8, 16 x 16 or 32 x 32 - e.g. /2 on 32 x 32 (every released preset) or 64 x 64, /4 on 64 x 64 or 32 x 32, /8 on 32 x 32.
-    if (desc->patch_size != 2 && desc->patch_size != 4 && desc->patch_size != 8)
+    if (!dit_patch_ok(desc->patch_size))
         return fail(nullptr, "lfm_create: patch_size must be 2, 4 or 8 (got %d)", desc->patch_size);
     {
         const int g = desc->img_resolution / desc->patch_size;
@@ -527,11 +537,8 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
             return fail(nullptr, "lfm_create: the token grid (img_resolution / patch_size) must be 4, 8, 16 or 32 per side, i.e. 16, 64, "
                         "256 or 1024 tokens (got img_resolution %d, patch_size %d)", desc->img_resolution, desc->patch_size);
     }
-    {
-        const int nv = desc->hidden_size / 128;
-        if (desc->hidden_size % 128 != 0 || !(nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9))
-            return fail(nullptr, "lfm_create: hidden_size must be one of 256, 384, 768, 1024, 1152 (got %d)", desc->hidden_size);
-    }
+    if (!ln_width_ok(desc->hidden_size))
+        return fail(nullptr, "lfm_create: hidden_size must be one of 256, 384, 768, 1024, 1152 (got %d)", desc->hidden_size);
     if (desc->num_heads <= 0 || (desc->num_heads * 64 != desc->hidden_size && desc->num_heads * 72 != desc->hidden_size))
         return fail(nullptr, "lfm_create: head_dim must be 64 or 72 (hidden %d, heads %d)", desc->hidden_size, desc->num_heads);
     if (desc->mlp_hidden % 64 != 0) return fail(nullptr, "lfm_create: mlp_hidden must be a multiple of 64");
@@ -573,15 +580,62 @@ extern "C" int lfm_set_fp8(lfm_ctx* ctx, int enable) {
     ctx->fp8 = on;
     for (int i = 0; i < ctx->L; ++i) {
         BlockW& b = ctx->blk[i];
-        if (dev_free(ctx, b.w_qkv) || dev_free(ctx, b.w_fc1) || dev_free(ctx, b.q_qkv) || dev_free(ctx, b.s_qkv) ||
-            dev_free(ctx, b.q_fc1) || dev_free(ctx, b.s_fc1))
+        if (dev_free(ctx, b.w_qkv) || dev_free(ctx, b.w_fc1) || dev_free(ctx, b.s_qkv) || dev_free(ctx, b.s_fc1) ||
+            dit_register_ln_gemm_weights(ctx, i))
             return 1;
-        b.w_qkv = b.w_fc1 = nullptr;
-        b.q_qkv = b.q_fc1 = nullptr;
-        b.s_qkv = b.s_fc1 = nullptr;
-        if (dit_register_ln_gemm_weights(ctx, i)) return 1;
     }
     return 0;
+}
+
+// The matrix slot s's layout makes of its source, [rows, cols]: what E4M3_ROWS quantises row by row.
+static std::pair<int, int> laid_out_dims(const ParamSlot& s) {
+    const int r0 = static_cast<int>(s.shape[0]), rest = static_cast<int>(s.numel / r0);
+    switch (s.layout) {
+        case Layout::TRANSPOSE: return {rest, r0};
+        case Layout::QKV_W: return {3 * (r0 / 3 / s.aux[0]) * s.aux[1], rest};  // 3 heads dhp rows
+        case Layout::QKV_B: return {1, 3 * (r0 / 3 / s.aux[0]) * s.aux[1]};
+        case Layout::PROJ_PAD: return {r0, r0 / s.aux[0] * s.aux[1]};  // heads dhp columns
+        default: return {r0, rest};
+    }
+}
+
+// Slot s's layout of the fp32 source src into out, [rows, cols] as bf16 (out_bf16) or fp32, on the default stream.  CONV and PROJ_PAD
+// have bf16 kernels only, TRANSPOSE and QKV_B fp32 ones: cudaErrorInvalidValue for the other type.
+static cudaError_t launch_layout(const ParamSlot& s, const float* src, void* out, bool out_bf16, int rows, int cols) {
+    const size_t n = static_cast<size_t>(rows) * cols;
+    const unsigned grid = blocks_for(n);
+    const int r0 = static_cast<int>(s.shape[0]), K = static_cast<int>(s.numel / r0), dh = s.aux[0], dhp = s.aux[1];
+    auto* ob = static_cast<__nv_bfloat16*>(out);
+    auto* of = static_cast<float*>(out);
+    switch (s.layout) {
+        case Layout::COPY:
+            if (!out_bf16) return cudaMemcpyAsync(of, src, n * sizeof(float), cudaMemcpyDeviceToDevice);
+            f32_to_bf16_kernel<<<blocks_for((n + 3) / 4), 256>>>(src, ob, n);
+            return cudaSuccess;
+        case Layout::QKV_W:  // 3 heads dhp rows
+            if (out_bf16) qkv_weight_reorder_kernel<<<grid, 256>>>(src, ob, K, r0 / 3 / dh, dh, dhp, s.aux[2], s.aux[3]);
+            else qkv_weight_reorder_kernel<<<grid, 256>>>(src, of, K, r0 / 3 / dh, dh, dhp, s.aux[2], s.aux[3]);
+            return cudaSuccess;
+        case Layout::CONV:
+            if (!out_bf16) break;
+            conv_weight_repack_kernel<<<grid, 256>>>(src, ob, r0, static_cast<int>(s.shape[1]), static_cast<int>(s.shape[2] * s.shape[3]));
+            return cudaSuccess;
+        case Layout::PROJ_PAD:
+            if (!out_bf16) break;
+            dit_proj_weight_pad_kernel<<<grid, 256>>>(src, ob, r0, dh, dhp);
+            return cudaSuccess;
+        case Layout::TRANSPOSE:
+            if (out_bf16) break;
+            transpose_f32_kernel<<<grid, 256>>>(src, of, r0, K);
+            return cudaSuccess;
+        case Layout::QKV_B:
+            if (out_bf16) break;
+            qkv_bias_reorder_kernel<<<grid, 256>>>(src, of, r0 / 3 / dh, dh, dhp, s.aux[2], s.aux[3]);
+            return cudaSuccess;
+        case Layout::RESAMPLE_FILTER:
+            break;
+    }
+    return cudaErrorInvalidValue;
 }
 
 extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int dtype, const int64_t* shape, int ndim) {
@@ -595,83 +649,36 @@ extern "C" int lfm_set_param(lfm_ctx* ctx, const char* key, const void* ptr, int
         if (shape[i] != s.shape[i])
             return fail(ctx, "lfm_set_param(%s): dim %d is %lld, expected %lld", key, i, (long long)shape[i], (long long)s.shape[i]);
     if (bind(ctx)) return 1;
-    if (s.xform == Xform::F32) {
+    if (s.layout == Layout::COPY && s.store == Store::F32) {
         CUDA_OK(cudaMemcpy(s.dst, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
-    } else {
-        // QKV_W_E4M3 re-orders into fp32 behind the source: 3 heads dhp rows of K
-        const size_t reordered = s.xform == Xform::QKV_W_E4M3
-                                     ? static_cast<size_t>(3) * (s.shape[0] / 3 / s.aux[0]) * s.aux[1] * (s.numel / s.shape[0])
-                                     : 0;
-        const size_t need = s.numel + reordered;
-        if (ctx->staging_elems < need) {
-            if (ctx->staging != nullptr) CUDA_OK(cudaFree(ctx->staging));
-            ctx->staging = nullptr;
-            CUDA_OK(cudaMalloc(&ctx->staging, need * sizeof(float)));
-            ctx->staging_elems = need;
-        }
-        CUDA_OK(cudaMemcpy(ctx->staging, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
-        switch (s.xform) {
-            case Xform::F32:
-                break;
-            case Xform::BF16:
-                f32_to_bf16_kernel<<<blocks_for((s.numel + 3) / 4), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), s.numel);
-                break;
-            case Xform::CONV_BF16: {
-                const int taps = static_cast<int>(s.shape[2] * s.shape[3]);
-                conv_weight_repack_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst),
-                                                                       static_cast<int>(s.shape[0]), static_cast<int>(s.shape[1]), taps);
-                break;
-            }
-            case Xform::TRANSPOSE_F32: {
-                const int r0 = static_cast<int>(s.shape[0]);
-                transpose_f32_kernel<<<blocks_for(s.numel), 256>>>(ctx->staging, static_cast<float*>(s.dst), r0,
-                                                                  static_cast<int>(s.numel / r0));
-                break;
-            }
-            case Xform::QKV_W:
-            case Xform::QKV_B: {  // the destination has 3 heads dhp rows
-                const int dh = s.aux[0], dhp = s.aux[1], heads = static_cast<int>(s.shape[0] / 3) / dh;
-                const int K = static_cast<int>(s.numel / s.shape[0]);
-                const size_t out_n = static_cast<size_t>(3) * heads * dhp * K;
-                if (s.xform == Xform::QKV_W)
-                    qkv_weight_reorder_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), K, heads, dh, dhp,
-                                                                          s.aux[2], s.aux[3]);
-                else
-                    qkv_bias_reorder_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<float*>(s.dst), heads, dh, dhp, s.aux[2],
-                                                                        s.aux[3]);
-                break;
-            }
-            case Xform::RESAMPLE_FILTER: {
-                float h[4] = {0.f, 0.f, 0.f, 0.f};
-                CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
-                for (float v : h)
-                    if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
-                break;
-            }
-            case Xform::QKV_W_E4M3: {
-                const int dh = s.aux[0], dhp = s.aux[1], heads = static_cast<int>(s.shape[0] / 3) / dh;
-                const int K = static_cast<int>(s.numel / s.shape[0]);
-                float* tmp = ctx->staging + s.numel;
-                qkv_weight_reorder_kernel<<<blocks_for(reordered), 256>>>(ctx->staging, tmp, K, heads, dh, dhp, s.aux[2], s.aux[3]);
-                launch_quantize_rows_e4m3(nullptr, tmp, static_cast<__nv_fp8_e4m3*>(s.dst), s.row_scale, 3 * heads * dhp, K);
-                break;
-            }
-            case Xform::E4M3_ROWS: {
-                const int N = static_cast<int>(s.shape[0]);
-                launch_quantize_rows_e4m3(nullptr, ctx->staging, static_cast<__nv_fp8_e4m3*>(s.dst), s.row_scale, N,
-                                          static_cast<int>(s.numel / N));
-                break;
-            }
-            case Xform::DIT_PROJ_PAD: {
-                const int Dm = static_cast<int>(s.shape[0]);
-                const size_t out_n = static_cast<size_t>(Dm) * (Dm / s.aux[0]) * s.aux[1];
-                dit_proj_weight_pad_kernel<<<blocks_for(out_n), 256>>>(ctx->staging, static_cast<__nv_bfloat16*>(s.dst), Dm, s.aux[0], s.aux[1]);
-                break;
-            }
-        }
-        CUDA_OK(cudaGetLastError());
-        CUDA_OK(cudaDeviceSynchronize());
+        s.set = true;
+        return 0;
     }
+    // Every other transform reads the source from the staging buffer.  For E4M3_ROWS the layout writes fp32 behind the source,
+    // and the rows of that matrix are quantised into the destination.
+    const bool e4m3 = s.store == Store::E4M3_ROWS;
+    const auto [rows, cols] = laid_out_dims(s);
+    const size_t need = s.numel + (e4m3 ? static_cast<size_t>(rows) * cols : 0);
+    if (ctx->staging_elems < need) {
+        if (ctx->staging != nullptr) CUDA_OK(cudaFree(ctx->staging));
+        ctx->staging = nullptr;
+        CUDA_OK(cudaMalloc(&ctx->staging, need * sizeof(float)));
+        ctx->staging_elems = need;
+    }
+    CUDA_OK(cudaMemcpy(ctx->staging, ptr, s.numel * sizeof(float), cudaMemcpyDefault));
+    if (s.layout == Layout::RESAMPLE_FILTER) {
+        float h[4] = {0.f, 0.f, 0.f, 0.f};
+        CUDA_OK(cudaMemcpy(h, ctx->staging, sizeof(h), cudaMemcpyDeviceToHost));
+        for (float v : h)
+            if (v != 0.25f) return fail(ctx, "lfm_set_param(%s): resample_filter must be [[0.25, 0.25], [0.25, 0.25]] (EDM.py:96-98)", key);
+    } else {
+        float* laid = ctx->staging + s.numel;  // E4M3_ROWS only
+        if (launch_layout(s, ctx->staging, e4m3 ? laid : s.dst, s.store == Store::BF16, rows, cols) != cudaSuccess)
+            return fail(ctx, "lfm_set_param(%s): no kernel for this layout and storage type", key);
+        if (e4m3) launch_quantize_rows_e4m3(nullptr, laid, static_cast<__nv_fp8_e4m3*>(s.dst), s.row_scale, rows, cols);
+    }
+    CUDA_OK(cudaGetLastError());
+    CUDA_OK(cudaDeviceSynchronize());
     s.set = true;
     return 0;
 }
@@ -700,6 +707,13 @@ static int alloc_solver_state(lfm_ctx* ctx, int R) {
 
 static int unet_finalize(lfm_ctx* ctx, int R);
 
+// The element type of the DiT's LayerNorm-fed GEMM operands, xn and the qkv / fc1 weights: f(__nv_bfloat16{}), or in FP8 mode
+// f(__nv_fp8_e4m3{}).  The one place lfm_finalize and the forward choose it.
+template <typename F>
+static int with_ln_operand(const lfm_ctx* ctx, F&& f) {
+    return ctx->fp8 ? f(__nv_fp8_e4m3{}) : f(__nv_bfloat16{});
+}
+
 extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (ctx == nullptr) return fail(ctx, "lfm_finalize: null ctx");
     if (max_batch < 1) return fail(ctx, "lfm_finalize: max_batch must be >= 1");
@@ -719,11 +733,18 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     const size_t M = (size_t)R * T;
     const int Rpad = R < 128 ? 128 : R;
     if (dev_alloc(ctx, &ctx->x_tok, M * D)) return 1;
-    if (ctx->fp8) {
-        if (dev_alloc(ctx, &ctx->xn8, M * D) || dev_alloc(ctx, &ctx->xn_scale, M)) return 1;
-    } else if (dev_alloc(ctx, &ctx->xn, M * D)) {
+    // xn (with its row scales for e4m3) and the tensor maps of the LayerNorm-fed GEMMs' operands
+    if (with_ln_operand(ctx, [&](auto op) {
+            using Op = decltype(op);
+            Op* xn = nullptr;
+            if (dev_alloc(ctx, &xn, M * D) || (std::is_same_v<Op, __nv_fp8_e4m3> && dev_alloc(ctx, &ctx->xn_scale, M))) return 1;
+            ctx->xn = xn;
+            bool ok = make_tmap_operand<Op>(&ctx->tm_xn, xn, M, D);
+            for (auto& b : ctx->blk)
+                ok = ok && make_tmap_operand<Op>(&b.tm_qkv, b.w_qkv, 3 * Dq, D) && make_tmap_operand<Op>(&b.tm_fc1, b.w_fc1, Hd, D);
+            return ok ? 0 : fail(ctx, "lfm_finalize: cuTensorMapEncodeTiled failed");
+        }))
         return 1;
-    }
     if (dev_alloc(ctx, &ctx->qkv, M * 3 * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->attn, M * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->hmid, M * Hd)) return 1;
@@ -734,9 +755,7 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (dev_alloc(ctx, &ctx->v_net, (size_t)R * ctx->out_chw)) return 1;
     if (alloc_solver_state(ctx, R)) return 1;
 
-    bool ok = true;
-    ok &= ctx->fp8 ? make_tmap_e4m3(&ctx->tm_xn, ctx->xn8, M, D, kGemmBoxRows) : make_tmap_bf16(&ctx->tm_xn, ctx->xn, M, D, kGemmBoxRows);
-    ok &= make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, kGemmBoxRows);
+    bool ok = make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, kGemmBoxRows);
@@ -746,13 +765,6 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     ok &= make_tmap_out(&ctx->tmo_x_tok, ctx->x_tok, M, D, D, true);
     ok &= make_tmap_out(&ctx->tmo_mod, ctx->mod, R, ctx->Nmod, ctx->Nmod, true);
     for (auto& b : ctx->blk) {
-        if (ctx->fp8) {
-            ok &= make_tmap_e4m3(&b.tm_qkv, b.q_qkv, 3 * Dq, D, kGemmBoxRows);
-            ok &= make_tmap_e4m3(&b.tm_fc1, b.q_fc1, Hd, D, kGemmBoxRows);
-        } else {
-            ok &= make_tmap_bf16(&b.tm_qkv, b.w_qkv, 3 * Dq, D, kGemmBoxRows);
-            ok &= make_tmap_bf16(&b.tm_fc1, b.w_fc1, Hd, D, kGemmBoxRows);
-        }
         ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, kGemmBoxRows);
         ok &= make_tmap_bf16(&b.tm_fc2, b.w_fc2, D, Hd, kGemmBoxRows);
     }
@@ -784,7 +796,8 @@ static int check_ready(lfm_ctx* ctx, int rows, const char* who);
 
 // The DiT's conditioning for `rows` rows (models/DiT.py:125,264): tf = timestep features of t (t_numel 1 broadcasts),
 // h1 = SiLU(mlp.0(tf)) (fp32), c = SiLU(mlp.2(h1) + table[y]) (bf16, the adaLN GEMM's operand).  y NULL reads the null row
-// table_rows - 1.  w0 [D, 256], w2 [D, D]: D / 128 <= 9 float4 per lane (skinny_linear_kernel).
+// table_rows - 1.  w0 [D, 256], w2 [D, D]: D a multiple of 128 up to kConditionMaxD.
+constexpr int kConditionMaxD = 9 * 128;  // skinny_linear_kernel holds a weight row in 9 float4 per lane (its MAXV)
 static int launch_dit_condition(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const long long* y, int rows, int D,
                                 const float* w0, const float* b0, const float* w2, const float* b2, const float* table,
                                 int table_rows, float* tf, float* h1, __nv_bfloat16* c) {
@@ -813,10 +826,11 @@ static int launch_patch_embed(lfm_ctx* ctx, cudaStream_t s, const float* x, int 
 
 // FinalLayer + unpatchify of M token rows into v_net (NCHW fp32): the specialised kernel (16 x D weight in shared memory) for
 // p = 2 (C = 4), the generic one for p = 4 and 8.  At most 2 blocks per SM; each warp loops over the rows beyond.
+constexpr int kFinalLayerMaxD = 1536;  // widest D whose 16 x D weight fits the specialised kernel's shared memory (96 KB)
 static int launch_final_layer(lfm_ctx* ctx, cudaStream_t s, const float* x, const float* shift, const float* scale, int mod_stride,
                               const float* W, const float* bias, float* v_net, int M, int D, int G, int C, int p) {
     static DevOnce once;
-    CUDA_OK(smem_opt_in(once, final_layer_kernel, 16 * 1536 * 4));  // largest supported width (hidden_size <= 1536)
+    CUDA_OK(smem_opt_in(once, final_layer_kernel, 16 * kFinalLayerMaxD * (int)sizeof(float)));
     int grid = (M + 7) / 8;
     if (grid > 2 * g_num_sms) grid = 2 * g_num_sms;
     if (p == 2)
@@ -856,27 +870,26 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
         dir ^= 1;
         return d;
     };
-    // LayerNorm + modulate into xn, and the GEMM that reads it (qkv, fc1): bf16, or e4m3 with row scales in FP8 mode
-    auto ln = [&](const float* shift, const float* scale) {
-        const int d = next_dir();
-        return ctx->fp8 ? launch_ln(s, ctx->x_tok, ctx->xn8, shift, scale, Nmod, T, M, D, d, ctx->xn_scale)
-                        : launch_ln(s, ctx->x_tok, ctx->xn, shift, scale, Nmod, T, M, D, d);
-    };
-    auto ln_gemm = [&](const CUtensorMap& tw, const float* w_scale, int N, int epi, GemmEpi ep) {
+    // LayerNorm + modulate of x_tok into xn, then the GEMM that reads xn (qkv, fc1), in the operand type of the mode
+    auto ln_gemm = [&](const float* shift, const float* scale, const CUtensorMap& tw, const float* w_scale, int N, int epi, GemmEpi ep) {
+        const int ln_dir = next_dir();
         ep.reverse_m = next_dir();
-        if (!ctx->fp8) return launch_gemm(s, ctx->tm_xn, tw, M, N, D, epi, 0, ep);
         ep.a_scale = ctx->xn_scale;
         ep.w_scale = w_scale;
-        return launch_gemm<__nv_fp8_e4m3>(s, ctx->tm_xn, tw, M, N, D, epi, 0, ep);
+        return with_ln_operand(ctx, [&](auto op) {
+            using Op = decltype(op);
+            COUNT_LAUNCH(launch_ln(s, ctx->x_tok, static_cast<Op*>(ctx->xn), shift, scale, Nmod, T, M, D, ln_dir, ctx->xn_scale));
+            COUNT_LAUNCH(launch_gemm<Op>(s, ctx->tm_xn, tw, M, N, D, epi, 0, ep));
+            return 0;
+        });
     };
     for (int l = 0; l < L; ++l) {
         BlockW& b = ctx->blk[l];
         const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
-        COUNT_LAUNCH(ln(mb, mb + D));
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
             ep.out_map = &ctx->tmo_qkv;
-            COUNT_LAUNCH(ln_gemm(b.tm_qkv, b.s_qkv, 3 * Dq, EPI_BIAS_BF16, ep));
+            if (ln_gemm(mb, mb + D, b.tm_qkv, b.s_qkv, 3 * Dq, EPI_BIAS_BF16, ep)) return 1;
         }
         {
             next_dir();  // attention reads each (sample, head) once: the sweep direction only keeps the GEMMs alternating
@@ -888,11 +901,10 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
             ep.out_map = &ctx->tmo_x_tok;
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_attn, b.tm_proj, M, D, Dq, EPI_GATE_RESID_F32, 0, ep));
         }
-        COUNT_LAUNCH(ln(mb + 3 * D, mb + 4 * D));
         {
             GemmEpi ep{b.b_fc1, ctx->hmid, Hd, nullptr, 0, T};
             ep.out_map = &ctx->tmo_hmid;
-            COUNT_LAUNCH(ln_gemm(b.tm_fc1, b.s_fc1, Hd, EPI_BIAS_GELU_BF16, ep));
+            if (ln_gemm(mb + 3 * D, mb + 4 * D, b.tm_fc1, b.s_fc1, Hd, EPI_BIAS_GELU_BF16, ep)) return 1;
         }
         {
             GemmEpi ep{b.b_fc2, ctx->x_tok, D, mb + 5 * D, Nmod, T};  // x += gate_mlp * fc2(...)   (models/DiT.py:130)
@@ -1479,27 +1491,38 @@ static int dbg_run(Op&& op) {
     return op(&dbg);
 }
 
-// lfm_dbg_gemm and lfm_dbg_gemm_reversed: `reverse` sets GemmEpi::reverse_m, as the network does on every other GEMM.
-// lfm_dbg_gemm_path: tma_store = 0 / 1 forces the epilogue's stores.  By default (-1) the output is stored through a tensor map
-// whenever one can be made for it (16-byte aligned base and pitch), as in the network.
-static int dbg_gemm(const char* who, int reverse, const void* a_bf16, const void* w_bf16, const float* bias, void* out, const float* gate,
-                    int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream,
-                    int tma_store = -1) {
-    if (K % 64 != 0 || N % 8 != 0) return fail(nullptr, "%s: K must be a multiple of 64 and N of 8", who);
+// The GEMM entries' body: lfm_dbg_gemm, _reversed and _path on bf16 operands, lfm_dbg_gemm_fp8 (Op = __nv_fp8_e4m3) on e4m3 ones with
+// their row scales a_scale and w_scale.  `reverse` sets GemmEpi::reverse_m, as the network does on every other GEMM.  tma_store = 0 / 1
+// forces the epilogue's stores.  By default (-1) the output is stored through a tensor map whenever one can be made for it (16-byte
+// aligned base and pitch), as in the network.
+template <typename Op = __nv_bfloat16>
+static int dbg_gemm(const char* who, int reverse, const void* a, const void* w, const float* bias, void* out, const float* gate,
+                    int gate_stride, int rows_per_sample, int M, int N, int K, int epi, int block_n, void* stream, int tma_store = -1,
+                    const float* a_scale = nullptr, const float* w_scale = nullptr) {
+    constexpr bool e4m3 = std::is_same_v<Op, __nv_fp8_e4m3>;
+    if (M < 1 || N < 8 || N % 8 != 0 || K < 1 || K % gemm_block_k<Op>() != 0)
+        return fail(nullptr, "%s: K, M or N out of range: M must be >= 1, N a positive multiple of 8 and K of %d (got M %d, N %d, K %d)",
+                    who, gemm_block_k<Op>(), M, N, K);
+    if (e4m3 && epi != EPI_BIAS_BF16 && epi != EPI_BIAS_GELU_BF16)
+        return fail(nullptr, "%s: epi must be 0 (bias -> bf16) or 1 (bias + GELU -> bf16) (got %d)", who, epi);
     if (epi < EPI_BIAS_BF16 || epi > EPI_BIAS_F32) return fail(nullptr, "%s: unknown epilogue %d", who, epi);
     if (block_n != 0 && block_n != 128 && block_n != 256)
         return fail(nullptr, "%s: block_n must be 0, 128 or 256 (got %d)", who, block_n);
     if (tma_store < -1 || tma_store > 1) return fail(nullptr, "%s: tma_store must be -1, 0 or 1 (got %d)", who, tma_store);
+    if (e4m3 && (a == nullptr || a_scale == nullptr || w == nullptr || w_scale == nullptr || out == nullptr))
+        return fail(nullptr, "%s: a, a_scale, w, w_scale and out must not be NULL (bias may be)", who);
     return dbg_run([&](lfm_ctx* ctx) {
         CUtensorMap ta, tb, tc;
-        if (!make_tmap_bf16(&ta, a_bf16, M, K, kGemmBoxRows) || !make_tmap_bf16(&tb, w_bf16, N, K, kGemmBoxRows))
+        if (!make_tmap_operand<Op>(&ta, a, M, K) || !make_tmap_operand<Op>(&tb, w, N, K))
             return fail(ctx, "%s: tensor map encode failed", who);
         const bool has_c = tma_store != 0 && make_tmap_out(&tc, out, M, N, N, epi >= EPI_GATE_RESID_F32);
         if (tma_store == 1 && !has_c) return fail(ctx, "%s: no output tensor map for this output (16-byte alignment)", who);
         GemmEpi ep{bias, out, N, gate, gate_stride, rows_per_sample > 0 ? rows_per_sample : 1};
         ep.reverse_m = reverse;
         ep.out_map = has_c ? &tc : nullptr;
-        CUDA_OK(launch_gemm(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
+        ep.a_scale = a_scale;
+        ep.w_scale = w_scale;
+        CUDA_OK(launch_gemm<Op>(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
         return 0;
     });
 }
@@ -1528,73 +1551,47 @@ extern "C" int lfm_dbg_gemm_path(const void* a_bf16, const void* w_bf16, const f
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* shift, const float* scale, int mod_stride,
-                                   int rows_per_sample, int M, int D, int down, void* stream) {
-    const int nv = D / 128;
-    if (D % 128 != 0 || !(nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9))
-        return fail(nullptr, "lfm_dbg_ln_modulate: D must be 128 x {2, 3, 6, 8, 9} (got %d)", D);
-    if (rows_per_sample < kLnRows || rows_per_sample % kLnRows != 0)
-        return fail(nullptr, "lfm_dbg_ln_modulate: rows_per_sample must be a positive multiple of %d (got %d)", kLnRows, rows_per_sample);
-    if (M < 1) return fail(nullptr, "lfm_dbg_ln_modulate: M must be >= 1 (got %d)", M);
+// The body of lfm_dbg_ln_modulate (OutT = bf16) and lfm_dbg_ln_modulate_fp8 (e4m3 codes and their row scales ys).
+template <typename OutT>
+static int dbg_ln_modulate(const char* who, const float* x, void* y, float* ys, const float* shift, const float* scale, int mod_stride,
+                           int rows_per_sample, int M, int D, int down, void* stream) {
+    constexpr bool e4m3 = std::is_same_v<OutT, __nv_fp8_e4m3>;
+    if (!ln_width_ok(D)) return fail(nullptr, "%s: D must be 128 x {2, 3, 6, 8, 9} (got %d)", who, D);
+    if (!ln_rows_per_sample_ok(rows_per_sample))
+        return fail(nullptr, "%s: rows_per_sample must be a positive multiple of %d (got %d)", who, kLnRows, rows_per_sample);
+    if (M < 1) return fail(nullptr, "%s: M must be >= 1 (got %d)", who, M);
     if (mod_stride < 0 || mod_stride % 4 != 0)
-        return fail(nullptr, "lfm_dbg_ln_modulate: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
-    if (down != 0 && down != 1) return fail(nullptr, "lfm_dbg_ln_modulate: down must be 0 or 1 (got %d)", down);
-    if (!aligned16(x) || !aligned16(shift) || !aligned16(scale) || !aligned16(y_bf16) || x == nullptr || y_bf16 == nullptr ||
-        shift == nullptr || scale == nullptr)
-        return fail(nullptr, "lfm_dbg_ln_modulate: x, y, shift and scale must not be NULL and must be 16-byte aligned");
+        return fail(nullptr, "%s: mod_stride must be a non-negative multiple of 4 (got %d)", who, mod_stride);
+    if (down != 0 && down != 1) return fail(nullptr, "%s: down must be 0 or 1 (got %d)", who, down);
+    if (x == nullptr || y == nullptr || shift == nullptr || scale == nullptr || (e4m3 && ys == nullptr))
+        return fail(nullptr, "%s: x, y, %sshift and scale must not be NULL", who, e4m3 ? "y_scale, " : "");
+    if (!aligned16(x) || !aligned16(y) || !aligned16(shift) || !aligned16(scale))
+        return fail(nullptr, "%s: x, y, shift and scale must be 16-byte aligned", who);
     return dbg_run([&](lfm_ctx* ctx) {
-        COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<__nv_bfloat16*>(y_bf16), shift, scale, mod_stride,
-                               rows_per_sample, M, D, down));
+        COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<OutT*>(y), shift, scale, mod_stride, rows_per_sample, M,
+                               D, down, ys));
         return 0;
     });
+}
+
+extern "C" int lfm_dbg_ln_modulate(const float* x, void* y_bf16, const float* shift, const float* scale, int mod_stride,
+                                   int rows_per_sample, int M, int D, int down, void* stream) {
+    return dbg_ln_modulate<__nv_bfloat16>("lfm_dbg_ln_modulate", x, y_bf16, nullptr, shift, scale, mod_stride, rows_per_sample, M, D,
+                                          down, stream);
 }
 
 // The FP8 mode's kernels, through the launch helpers the DiT forward and lfm_set_param use.
 
 extern "C" int lfm_dbg_gemm_fp8(const void* a_e4m3, const float* a_scale, const void* w_e4m3, const float* w_scale, const float* bias,
                                 void* out_bf16, int M, int N, int K, int epi, int block_n, void* stream) {
-    if (M < 1 || N < 8 || N % 8 != 0 || K < 128 || K % 128 != 0)
-        return fail(nullptr, "lfm_dbg_gemm_fp8: M must be >= 1, N a positive multiple of 8 and K of 128 (got M %d, N %d, K %d)", M, N, K);
-    if (epi != EPI_BIAS_BF16 && epi != EPI_BIAS_GELU_BF16)
-        return fail(nullptr, "lfm_dbg_gemm_fp8: epi must be 0 (bias -> bf16) or 1 (bias + GELU -> bf16) (got %d)", epi);
-    if (block_n != 0 && block_n != 128 && block_n != 256)
-        return fail(nullptr, "lfm_dbg_gemm_fp8: block_n must be 0, 128 or 256 (got %d)", block_n);
-    if (a_e4m3 == nullptr || a_scale == nullptr || w_e4m3 == nullptr || w_scale == nullptr || out_bf16 == nullptr)
-        return fail(nullptr, "lfm_dbg_gemm_fp8: a, a_scale, w, w_scale and out must not be NULL (bias may be)");
-    return dbg_run([&](lfm_ctx* ctx) {
-        CUtensorMap ta, tb, tc;
-        if (!make_tmap_e4m3(&ta, a_e4m3, M, K, kGemmBoxRows) || !make_tmap_e4m3(&tb, w_e4m3, N, K, kGemmBoxRows))
-            return fail(ctx, "lfm_dbg_gemm_fp8: tensor map encode failed");
-        GemmEpi ep{bias, out_bf16, N, nullptr, 0, 1};
-        ep.out_map = make_tmap_out(&tc, out_bf16, M, N, N, false) ? &tc : nullptr;
-        ep.a_scale = a_scale;
-        ep.w_scale = w_scale;
-        COUNT_LAUNCH(launch_gemm<__nv_fp8_e4m3>(static_cast<cudaStream_t>(stream), ta, tb, M, N, K, epi, block_n, ep));
-        return 0;
-    });
+    return dbg_gemm<__nv_fp8_e4m3>("lfm_dbg_gemm_fp8", 0, a_e4m3, w_e4m3, bias, out_bf16, nullptr, 0, 1, M, N, K, epi, block_n, stream, -1,
+                                   a_scale, w_scale);
 }
 
 extern "C" int lfm_dbg_ln_modulate_fp8(const float* x, void* y_e4m3, float* y_scale, const float* shift, const float* scale, int mod_stride,
                                        int rows_per_sample, int M, int D, int down, void* stream) {
-    const int nv = D / 128;
-    if (D % 128 != 0 || !(nv == 2 || nv == 3 || nv == 6 || nv == 8 || nv == 9))
-        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: D must be 128 x {2, 3, 6, 8, 9} (got %d)", D);
-    if (rows_per_sample < kLnRows || rows_per_sample % kLnRows != 0)
-        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: rows_per_sample must be a positive multiple of %d (got %d)", kLnRows,
-                    rows_per_sample);
-    if (M < 1) return fail(nullptr, "lfm_dbg_ln_modulate_fp8: M must be >= 1 (got %d)", M);
-    if (mod_stride < 0 || mod_stride % 4 != 0)
-        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
-    if (down != 0 && down != 1) return fail(nullptr, "lfm_dbg_ln_modulate_fp8: down must be 0 or 1 (got %d)", down);
-    if (x == nullptr || y_e4m3 == nullptr || y_scale == nullptr || shift == nullptr || scale == nullptr || !aligned16(x) ||
-        !aligned16(y_e4m3) || !aligned16(shift) || !aligned16(scale))
-        return fail(nullptr, "lfm_dbg_ln_modulate_fp8: x, y, y_scale, shift and scale must not be NULL (x, y, shift and scale "
-                             "16-byte aligned)");
-    return dbg_run([&](lfm_ctx* ctx) {
-        COUNT_LAUNCH(launch_ln(static_cast<cudaStream_t>(stream), x, static_cast<__nv_fp8_e4m3*>(y_e4m3), shift, scale, mod_stride,
-                               rows_per_sample, M, D, down, y_scale));
-        return 0;
-    });
+    return dbg_ln_modulate<__nv_fp8_e4m3>("lfm_dbg_ln_modulate_fp8", x, y_e4m3, y_scale, shift, scale, mod_stride, rows_per_sample, M, D,
+                                          down, stream);
 }
 
 extern "C" int lfm_dbg_quantize_rows_fp8(const float* w, void* codes_e4m3, float* scales, int N, int K, void* stream) {
@@ -1614,8 +1611,8 @@ extern "C" int lfm_dbg_dit_condition(const float* t, int t_numel, const long lon
     if (rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: rows must be >= 1 (got %d)", rows);
     if (t_numel != 1 && t_numel != rows)
         return fail(nullptr, "lfm_dbg_dit_condition: t_numel must be 1 or rows (got %d, rows %d)", t_numel, rows);
-    if (D < 128 || D % 128 != 0 || D > 9 * 128)
-        return fail(nullptr, "lfm_dbg_dit_condition: D must be a multiple of 128 up to 1152 (got %d)", D);
+    if (D < 128 || D % 128 != 0 || D > kConditionMaxD)
+        return fail(nullptr, "lfm_dbg_dit_condition: D must be a multiple of 128 up to %d (got %d)", kConditionMaxD, D);
     if (table_rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: table_rows must be >= 1 (got %d)", table_rows);
     if (t == nullptr || w0 == nullptr || b0 == nullptr || w2 == nullptr || b2 == nullptr || table == nullptr || tf_out == nullptr ||
         h1_out == nullptr || c_bf16 == nullptr)
@@ -1625,8 +1622,6 @@ extern "C" int lfm_dbg_dit_condition(const float* t, int t_numel, const long lon
                                     tf_out, h1_out, static_cast<__nv_bfloat16*>(c_bf16));
     });
 }
-
-static bool dit_patch_ok(int p) { return p == 2 || p == 4 || p == 8; }
 
 extern "C" int lfm_dbg_patch_embed(const float* x, int x_rows, const float* Wt, const float* bias, const float* pos, float* tok, int D,
                                    int G, int C, int p, int M, void* stream) {
@@ -1648,8 +1643,8 @@ extern "C" int lfm_dbg_final_layer(const float* x, const float* shift, const flo
     if (!dit_patch_ok(p)) return fail(nullptr, "lfm_dbg_final_layer: p must be 2, 4 or 8 (got %d)", p);
     if (p == 2 ? C != 4 : C < 1)
         return fail(nullptr, "lfm_dbg_final_layer: C must be 4 at p = 2 (the kernel computes 16 outputs), >= 1 otherwise (got %d)", C);
-    if (D < 128 || D % 128 != 0 || D > 1536)
-        return fail(nullptr, "lfm_dbg_final_layer: D must be a multiple of 128 up to 1536 (got %d)", D);
+    if (D < 128 || D % 128 != 0 || D > kFinalLayerMaxD)
+        return fail(nullptr, "lfm_dbg_final_layer: D must be a multiple of 128 up to %d (got %d)", kFinalLayerMaxD, D);
     if (mod_stride < 0 || mod_stride % 4 != 0)
         return fail(nullptr, "lfm_dbg_final_layer: mod_stride must be a non-negative multiple of 4 (got %d)", mod_stride);
     if (G < 1 || M < 1) return fail(nullptr, "lfm_dbg_final_layer: G and M must be >= 1 (got %d, %d)", G, M);
