@@ -270,13 +270,15 @@ int lfm_dbg_ln_modulate_fp8(const float* x, void* y_e4m3, float* y_scale, const 
 /* The FP8 mode's weight quantiser: w fp32 [N, K] (device) -> scales fp32 [N] = amax|w[n, :]| / 448 (1 for an all-zero row) and
  * codes e4m3 [N, K] = e4m3(w / scales[n]) (round to nearest even, saturating). */
 int lfm_dbg_quantize_rows_fp8(const float* w, void* codes_e4m3, float* scales, int N, int K, void* stream);
-/* The DiT's conditioning for `rows` rows, each stage into a caller-allocated output: tf_out fp32 [rows, 256] timestep features
- * [cos | sin] of t (t_numel 1 or rows), h1_out fp32 [rows, D] = SiLU(w0 tf + b0), c_bf16 bf16 [rows, D] =
- * SiLU(w2 h1 + b2 + table[y[r]]), y NULL = the null row table_rows - 1 for every row.  w0 [D, 256], w2 [D, D], table
- * [table_rows, D], all fp32; D a multiple of 128 up to 1152. */
-int lfm_dbg_dit_condition(const float* t, int t_numel, const long long* y, int rows, int D, const float* w0, const float* b0,
-                          const float* w2, const float* b2, const float* table, int table_rows, float* tf_out, float* h1_out,
-                          void* c_bf16, void* stream);
+/* The conditioning stage of the DiT, ADM and EDM networks for `rows` rows, each step into a caller-allocated output: tf_out fp32
+ * [rows, feat] timestep features [cos | sin] of t (t_numel 1 or rows), h1_out fp32 [rows, E] = SiLU(w0 tf + b0), c_bf16 bf16
+ * [rows, E] = SiLU(w2 h1 + b2 + table[row]) with row = y ? clamp(y[r], 0, max_row) : null_row, and no table term when that is
+ * -1.  The networks use max_row = null_row = table_rows - 1 (DiT), max_row = num_classes - 1 with null_row -1 (ADM), and
+ * max_row = label_dim, the all-zero row after the labels, with null_row -1 (EDM).  w0 [E, feat], w2 [E, E], table [max_row + 1, E],
+ * all fp32; feat and E multiples of 128 up to 4096.  table may be NULL when neither y nor null_row reads it. */
+int lfm_dbg_condition(const float* t, int t_numel, const long long* y, int rows, int feat, int E, const float* w0, const float* b0,
+                      const float* w2, const float* b2, const float* table, int max_row, int null_row, float* tf_out, float* h1_out,
+                      void* c_bf16, void* stream);
 /* The DiT's patch embed: M token rows of G x G tokens per sample, row m of sample b = m / G^2 reads latent b % x_rows of x (NCHW
  * fp32, C channels of side p G).  Wt fp32 [C p p, D] (the conv weight transposed, patch vector order (c, p, q)), bias [D],
  * pos [G^2, D] -> tok fp32 [M, D].  p 2 (C 4), 4 or 8; D a multiple of 4. */

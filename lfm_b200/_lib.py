@@ -74,7 +74,7 @@ SYMBOLS = {
     "lfm_dbg_gemm_fp8": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_ln_modulate_fp8": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_quantize_rows_fp8": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P]),
-    "lfm_dbg_dit_condition": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
+    "lfm_dbg_condition": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "lfm_dbg_patch_embed": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_final_layer": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "lfm_dbg_attention": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

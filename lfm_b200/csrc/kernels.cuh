@@ -7,65 +7,77 @@
 namespace lfm {
 
 // ------------------------------------------------------------------------------------------------
-// K2: sinusoidal timestep features  tf[b, :] = [cos(t f_i) | sin(t f_i)], f_i = exp(-ln(1e4) i / 128)
-// (reference models/DiT.py:43-62; raw t in [0,1], cos first).  t_numel == 1 broadcasts.
-__global__ void timestep_features_kernel(const float* __restrict__ t, int t_numel, float* __restrict__ tf, int B) {
+// The conditioning stage of every velocity network (DiT t_embedder / y_embedder, models/DiT.py:43-62,125,264; the UNets'
+// time_embed / label_emb, unet.py:613-624, and map_layer0 / map_layer1 / map_label, EDM.py:812-829), per network row:
+//   tf = [cos | sin](t f_k), f_k = exp(-ln(1e4) k / half)   (width 2 half, raw t, cos first; nn.py:103-121, DiT.py:43-62)
+//   h1 = SiLU(W0 tf + b0)                                     (fp32)
+//   c  = SiLU(W2 h1 + b2 + table[row])                        (bf16: the operand of the modulation GEMM)
+
+// Timestep features of width dim (even); t_numel == 1 broadcasts.  One block per row.
+__global__ void timestep_features_kernel(const float* __restrict__ t, int t_numel, float* __restrict__ tf, int dim) {
+    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
+    pdl_trigger();
     const int b = blockIdx.x;
-    const int i = threadIdx.x;  // 0..255
-    if (b >= B) return;
+    const int half = dim / 2;
     const float tv = t[t_numel == 1 ? 0 : b];
-    const int k = i & 127;
-    const float freq = expf(-9.210340371976184f * static_cast<float>(k) / 128.0f);
-    const float a = tv * freq;
-    tf[b * 256 + i] = (i < 128) ? cosf(a) : sinf(a);
+    for (int i = threadIdx.x; i < dim; i += blockDim.x) {
+        const int k = i < half ? i : i - half;
+        const float freq = expf(-9.210340371976184f * static_cast<float>(k) / static_cast<float>(half));
+        const float a = tv * freq;
+        tf[static_cast<size_t>(b) * dim + i] = (i < half) ? cosf(a) : sinf(a);
+    }
 }
 
-// ------------------------------------------------------------------------------------------------
-// K2/K3: skinny linear  out[b, j] = act( bias[j] + sum_k W[j, k] in[b, k] (+ table[idx[b], j]) )
-// One warp per output feature j; the weight row stays in registers while the warp sweeps the batch.
-// MODE 0: SiLU -> fp32 out          (t_embedder.mlp.0 + SiLU)
-// MODE 1: + label-embedding row, then SiLU -> bf16 out (c = t_emb + y_emb; adaLN's leading SiLU, DiT.py:125,264)
-template <int MODE>
+// One MLP layer of the stage: out[b, j] = SiLU(bias[j] + W[j, :] . in[b, :] (+ table[row, j])), W [N, K] fp32, K a multiple of 128.
+// One warp per output feature j: lane l accumulates the float4 m 32 + l of the row, m ascending, in one fmaf chain, then the warp
+// sums.  The first kCondRegV float4 of the lane's weights stay in registers while the warp sweeps the rows; a longer row streams
+// the rest from memory for every row.
+//   OutT float:          SiLU -> fp32 (h1)
+//   OutT __nv_bfloat16:  + the label row, SiLU -> bf16 (c).  row = idx ? clamp(idx[b], 0, max_row) : null_row; no table term
+//                        when that is negative.
+constexpr int kCondRegV = 9;  // K <= 1152 (every DiT width) runs from registers alone
+template <typename OutT>
 __global__ void __launch_bounds__(256)
-skinny_linear_kernel(const float* __restrict__ W, const float* __restrict__ bias, const float* __restrict__ in, int B,
-                     int N, int K, const float* __restrict__ table, const long long* __restrict__ idx, int null_row,
-                     float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16) {
-    constexpr int MAXV = 9;  // K <= 1152
+condition_mlp_kernel(const float* __restrict__ W, const float* __restrict__ bias, const float* __restrict__ in, int B, int N, int K,
+                     const float* __restrict__ table, const long long* __restrict__ idx, int max_row, int null_row,
+                     OutT* __restrict__ out) {
+    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
+    pdl_trigger();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int j = blockIdx.x * 8 + warp;
     if (j >= N) return;
     const int nv = K / 128;  // float4 per lane
-    float4 w[MAXV];
+    const float4* wp = reinterpret_cast<const float4*>(W + static_cast<size_t>(j) * K) + lane;
+    float4 w[kCondRegV];
 #pragma unroll
-    for (int m = 0; m < MAXV; ++m)
-        if (m < nv) w[m] = __ldg(reinterpret_cast<const float4*>(W + static_cast<size_t>(j) * K) + m * 32 + lane);
+    for (int m = 0; m < kCondRegV; ++m)
+        if (m < nv) w[m] = __ldg(wp + m * 32);
+    auto fma4 = [](float4 a, float4 x, float acc) {
+        acc = fmaf(a.x, x.x, acc);
+        acc = fmaf(a.y, x.y, acc);
+        acc = fmaf(a.z, x.z, acc);
+        return fmaf(a.w, x.w, acc);
+    };
     const float bj = bias[j];
     for (int b = 0; b < B; ++b) {
-        const float4* ip = reinterpret_cast<const float4*>(in + static_cast<size_t>(b) * K);
+        const float4* ip = reinterpret_cast<const float4*>(in + static_cast<size_t>(b) * K) + lane;
         float acc = 0.f;
 #pragma unroll
-        for (int m = 0; m < MAXV; ++m) {
-            if (m < nv) {
-                const float4 x = __ldg(ip + m * 32 + lane);
-                acc = fmaf(w[m].x, x.x, acc);
-                acc = fmaf(w[m].y, x.y, acc);
-                acc = fmaf(w[m].z, x.z, acc);
-                acc = fmaf(w[m].w, x.w, acc);
-            }
-        }
+        for (int m = 0; m < kCondRegV; ++m)
+            if (m < nv) acc = fma4(w[m], __ldg(ip + m * 32), acc);
+#pragma unroll 4  // fully unrolled, the tail's loads would take the registers of the weights above and spill
+        for (int m = kCondRegV; m < nv; ++m) acc = fma4(__ldg(wp + m * 32), __ldg(ip + m * 32), acc);
         acc = warp_sum(acc);
         if (lane == 0) {
             float v = acc + bj;
-            if (MODE == 1) {
-                long long row = (idx != nullptr) ? idx[b] : static_cast<long long>(null_row);
-                row = row < 0 ? 0 : (row > null_row ? null_row : row);  // never read outside the table (null_row = last row)
-                v += table[static_cast<size_t>(row) * N + j];
+            if constexpr (std::is_same_v<OutT, __nv_bfloat16>) {
+                long long row = null_row;
+                if (idx != nullptr) row = idx[b] < 0 ? 0 : (idx[b] > max_row ? max_row : idx[b]);  // never read outside the table
+                if (row >= 0) v += table[static_cast<size_t>(row) * N + j];
+                out[static_cast<size_t>(b) * N + j] = __float2bfloat16(silu(v));
+            } else {
+                out[static_cast<size_t>(b) * N + j] = silu(v);
             }
-            v = silu(v);
-            if (MODE == 0)
-                out_f32[static_cast<size_t>(b) * N + j] = v;
-            else
-                out_bf16[static_cast<size_t>(b) * N + j] = __float2bfloat16(v);
         }
     }
 }

@@ -296,13 +296,32 @@ struct BlockW {
 
 struct UNetState;
 
+// The conditioning stage of the DiT, ADM and EDM networks (kernels.cuh: timestep_features_kernel, condition_mlp_kernel): the
+// timestep MLP W0 [E, feat] and W2 [E, E], the label table with its label rule, and every layer's modulation rows (the DiT's adaLN,
+// the UNets' FiLM) concatenated into one weight [n_mod, E] for one GEMM.  cond_register, cond_finalize, cond_launch.
+struct Conditioning {
+    int feat = 0, E = 0;             // timestep-feature width and embedding width (E 0: the network has no stage)
+    int max_row = 0, null_row = -1;  // condition_mlp_kernel's label rule
+    int n_mod = 0, mod_rows = 0;     // rows of the modulation weight, and those registered so far (cond_add_mod)
+    float *w0 = nullptr, *b0 = nullptr, *w2 = nullptr, *b2 = nullptr, *table = nullptr, *b_mod = nullptr;
+    __nv_bfloat16* w_mod = nullptr;
+    // workspace: tf [R, feat], h1 [R, E], c_silu [max(R, 128), E], mod [R, n_mod]
+    float *tf = nullptr, *h1 = nullptr, *mod = nullptr;
+    __nv_bfloat16* c_silu = nullptr;
+    CUtensorMap tm_csilu, tm_wmod, tmo_mod;
+};
+// The K of both MLP layers (the feature width and E): condition_mlp_kernel reads a weight row as float4 per lane.  4096 is the widest
+// E = 4 model_channels that lfm_create_unet / lfm_create_edm admit (2 max(channel_mult) model_channels <= 2048).
+constexpr int kConditionMaxK = 4096;
+static bool condition_k_ok(int K) { return K >= 128 && K % 128 == 0 && K <= kConditionMaxK; }
+
 struct lfm_ctx {
     lfm_model_desc d{};
     NetKind net = NetKind::DIT;
     UNetState* un = nullptr;
     int device = 0;
     int num_sms = 0;
-    int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, Nmod = 0, HW = 0;
+    int D = 0, L = 0, H = 0, T = 0, G = 0, C = 0, Hd = 0, HW = 0;
     int in_chw = 0, out_chw = 0;  // floats of one image of the network input / of the solver state and the velocity
     int dh = 64, dhp = 64, Dq = 0;  // head_dim, its stored (zero-padded) width and the width H * dhp of the attention tensors
     int max_rows = 0;
@@ -316,20 +335,19 @@ struct lfm_ctx {
     float* staging = nullptr;
     size_t staging_elems = 0;
 
+    Conditioning cond;  // DiT, ADM and EDM
+
     // parameters
-    float *pos = nullptr, *pe_w = nullptr, *pe_b = nullptr, *t_w0 = nullptr, *t_b0 = nullptr, *t_w2 = nullptr,
-          *t_b2 = nullptr, *ytable = nullptr, *fin_w = nullptr, *fin_b = nullptr, *b_mod = nullptr;
-    __nv_bfloat16* w_mod = nullptr;
-    CUtensorMap tm_wmod;
+    float *pos = nullptr, *pe_w = nullptr, *pe_b = nullptr, *fin_w = nullptr, *fin_b = nullptr;
     std::vector<BlockW> blk;
 
     // workspace
-    float *x_tok = nullptr, *mod = nullptr, *tfreq = nullptr, *h1 = nullptr, *v_net = nullptr;
+    float *x_tok = nullptr, *v_net = nullptr;
     void* xn = nullptr;            // ln_modulate's output, in the operand type of the mode (with_ln_operand) ...
     float* xn_scale = nullptr;     // ... and its row scales (NULL for bf16)
-    __nv_bfloat16 *qkv = nullptr, *attn = nullptr, *hmid = nullptr, *c_silu = nullptr;
-    CUtensorMap tm_xn, tm_attn, tm_hmid, tm_csilu;
-    CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok, tmo_mod;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
+    __nv_bfloat16 *qkv = nullptr, *attn = nullptr, *hmid = nullptr;
+    CUtensorMap tm_xn, tm_attn, tm_hmid;
+    CUtensorMap tmo_qkv, tmo_hmid, tmo_x_tok;  // GEMM outputs (make_tmap_out): the TMA-store epilogue
     AttnOp attn_op;  // qkv -> attn of every block
 
     // solver state
@@ -398,6 +416,43 @@ static int alloc_param(lfm_ctx* ctx, const std::string& key, Tp** p, const std::
     if (dev_alloc(ctx, p, numel(shape))) return 1;
     add_param(ctx, key, *p, shape, layout, store, aux);
     return 0;
+}
+
+// The conditioning stage's parameters.  w0 / w2: the key prefixes of the two Linear layers ("<prefix>weight", "<prefix>bias");
+// table_key: the label table of table_rows labels (NULL: none), stored as given, [table_rows, E] (Layout::COPY), or transposed from a
+// bias-free Linear on a one-hot, [E, table_rows], with one all-zero row appended after the labels (Layout::TRANSPOSE, EDM's map_label:
+// the dropped label).  The label rule reads rows 0 .. max_row, the last label row (COPY) or the zero row (TRANSPOSE); null_row is
+// the row of y == NULL (-1: no table term).  n_mod: rows of the modulation weight, registered by the layers with cond_add_mod.
+static int cond_register(lfm_ctx* ctx, const std::string& w0, const std::string& w2, const char* table_key, int feat, int E,
+                         int table_rows, Layout table_layout, int null_row, int n_mod) {
+    Conditioning& c = ctx->cond;
+    if (!condition_k_ok(feat) || !condition_k_ok(E))
+        return fail(ctx, "conditioning: the feature width (%d) and the embedding width (%d) must be multiples of 128 up to %d", feat, E,
+                    kConditionMaxK);
+    c.feat = feat;
+    c.E = E;
+    c.n_mod = n_mod;
+    c.max_row = table_layout == Layout::TRANSPOSE ? table_rows : table_rows - 1;
+    c.null_row = null_row;
+    if (alloc_param(ctx, w0 + "weight", &c.w0, {E, feat}) || alloc_param(ctx, w0 + "bias", &c.b0, {E}) ||
+        alloc_param(ctx, w2 + "weight", &c.w2, {E, E}) || alloc_param(ctx, w2 + "bias", &c.b2, {E}))
+        return 1;
+    if (table_key != nullptr) {
+        const bool zero_row = table_layout == Layout::TRANSPOSE;
+        if (dev_alloc(ctx, &c.table, (size_t)(table_rows + zero_row) * E)) return 1;
+        add_param(ctx, table_key, c.table, zero_row ? std::vector<int64_t>{E, table_rows} : std::vector<int64_t>{table_rows, E}, table_layout);
+    }
+    return dev_alloc(ctx, &c.w_mod, (size_t)n_mod * E) || dev_alloc(ctx, &c.b_mod, n_mod);
+}
+// Registers a layer's modulation Linear (prefix "weight" [rows, E], "bias" [rows]) as the next `rows` rows of the stage's modulation
+// weight, and returns the offset of its rows in mod.
+static int cond_add_mod(lfm_ctx* ctx, const std::string& prefix, int rows) {
+    Conditioning& c = ctx->cond;
+    const int off = c.mod_rows;
+    add_param(ctx, prefix + "weight", c.w_mod + (size_t)off * c.E, {rows, c.E}, Layout::COPY, Store::BF16);
+    add_param(ctx, prefix + "bias", c.b_mod + off, {rows});
+    c.mod_rows += rows;
+    return off;
 }
 
 // Releases one allocation of ctx->allocs (a parameter storage replaced before lfm_finalize).
@@ -486,19 +541,14 @@ static int dit_register(lfm_ctx* ctx) {
     if (alloc_param(ctx, "pos_embed", &ctx->pos, {1, T, D}) ||
         alloc_param(ctx, "x_embedder.proj.weight", &ctx->pe_w, {D, 4, ps, ps}, Layout::TRANSPOSE) ||  // stored as [P, D]
         alloc_param(ctx, "x_embedder.proj.bias", &ctx->pe_b, {D}) ||
-        alloc_param(ctx, "t_embedder.mlp.0.weight", &ctx->t_w0, {D, 256}) ||
-        alloc_param(ctx, "t_embedder.mlp.0.bias", &ctx->t_b0, {D}) ||
-        alloc_param(ctx, "t_embedder.mlp.2.weight", &ctx->t_w2, {D, D}) ||
-        alloc_param(ctx, "t_embedder.mlp.2.bias", &ctx->t_b2, {D}) ||
-        alloc_param(ctx, "y_embedder.embedding_table.weight", &ctx->ytable, {d.table_rows, D}) ||
         alloc_param(ctx, "final_layer.linear.weight", &ctx->fin_w, {P, D}) ||
         alloc_param(ctx, "final_layer.linear.bias", &ctx->fin_b, {P}))
         return 1;
-    // all adaLN modulation layers in one table: block i at rows 6 i D, the final layer's after them
-    if (dev_alloc(ctx, &ctx->w_mod, (size_t)ctx->Nmod * D)) return 1;
-    if (dev_alloc(ctx, &ctx->b_mod, ctx->Nmod)) return 1;
-    add_param(ctx, "final_layer.adaLN_modulation.1.weight", ctx->w_mod + (size_t)6 * L * D * D, {2 * D, D}, Layout::COPY, Store::BF16);
-    add_param(ctx, "final_layer.adaLN_modulation.1.bias", ctx->b_mod + (size_t)6 * L * D, {2 * D});
+    // 256 frequencies (TimestepEmbedder, DiT.py:43-62); y NULL reads the last table row, the null class.  All adaLN modulation
+    // layers in one table: block i at rows 6 i D, the final layer's after them.
+    if (cond_register(ctx, "t_embedder.mlp.0.", "t_embedder.mlp.2.", "y_embedder.embedding_table.weight", 256, D, d.table_rows,
+                      Layout::COPY, d.table_rows - 1, (6 * L + 2) * D))
+        return 1;
     ctx->blk.resize(L);
     for (int i = 0; i < L; ++i) {
         BlockW& b = ctx->blk[i];
@@ -517,9 +567,9 @@ static int dit_register(lfm_ctx* ctx) {
             alloc_param(ctx, p + "mlp.fc2.weight", &b.w_fc2, {D, Hd}, Layout::COPY, Store::BF16) ||
             alloc_param(ctx, p + "mlp.fc2.bias", &b.b_fc2, {D}))
             return 1;
-        add_param(ctx, p + "adaLN_modulation.1.weight", ctx->w_mod + (size_t)i * 6 * D * D, {6 * D, D}, Layout::COPY, Store::BF16);
-        add_param(ctx, p + "adaLN_modulation.1.bias", ctx->b_mod + (size_t)i * 6 * D, {6 * D});
+        cond_add_mod(ctx, p + "adaLN_modulation.1.", 6 * D);
     }
+    cond_add_mod(ctx, "final_layer.adaLN_modulation.1.", 2 * D);
     return 0;
 }
 
@@ -554,7 +604,6 @@ extern "C" int lfm_create(const lfm_model_desc* desc, int device, lfm_ctx** out)
     ctx->Hd = desc->mlp_hidden;
     ctx->HW = desc->img_resolution;
     ctx->in_chw = ctx->out_chw = ctx->C * ctx->HW * ctx->HW;
-    ctx->Nmod = (6 * ctx->L + 2) * ctx->D;
     // head_dim 72 (DiT-XL) is stored padded to 80 channels; the qkv rows are stored in network_qkv_layout's order
     ctx->dh = desc->hidden_size / desc->num_heads;
     ctx->dhp = ctx->dh == 72 ? 80 : 64;
@@ -707,6 +756,20 @@ static int alloc_solver_state(lfm_ctx* ctx, int R) {
 
 static int unet_finalize(lfm_ctx* ctx, int R);
 
+// The conditioning stage's workspace for R rows and its tensor maps.  c_silu, the modulation GEMM's A operand, has at least the
+// 128 rows of one box.
+static int cond_finalize(lfm_ctx* ctx, int R) {
+    Conditioning& c = ctx->cond;
+    const int Rpad = R < 128 ? 128 : R;
+    if (dev_alloc(ctx, &c.tf, (size_t)R * c.feat) || dev_alloc(ctx, &c.h1, (size_t)R * c.E) || dev_alloc(ctx, &c.c_silu, (size_t)Rpad * c.E) ||
+        dev_alloc(ctx, &c.mod, (size_t)R * c.n_mod))
+        return 1;
+    bool ok = make_tmap_bf16(&c.tm_csilu, c.c_silu, Rpad, c.E, kGemmBoxRows);
+    ok &= make_tmap_bf16(&c.tm_wmod, c.w_mod, c.n_mod, c.E, kGemmBoxRows);
+    ok &= make_tmap_out(&c.tmo_mod, c.mod, R, c.n_mod, c.n_mod, true);
+    return ok ? 0 : fail(ctx, "lfm_finalize: cuTensorMapEncodeTiled failed (conditioning)");
+}
+
 // The element type of the DiT's LayerNorm-fed GEMM operands, xn and the qkv / fc1 weights: f(__nv_bfloat16{}), or in FP8 mode
 // f(__nv_fp8_e4m3{}).  The one place lfm_finalize and the forward choose it.
 template <typename F>
@@ -722,6 +785,7 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (ctx->finalized && max_batch <= ctx->max_rows) return 0;
     if (ctx->finalized) return fail(ctx, "lfm_finalize: already finalized for %d rows; create a new ctx for %d", ctx->max_rows, max_batch);
     if (bind(ctx)) return 1;
+    if (ctx->cond.E > 0 && cond_finalize(ctx, max_batch)) return 1;
     if (ctx->net != NetKind::DIT) {
         if (unet_finalize(ctx, max_batch)) return 1;
         if (alloc_solver_state(ctx, max_batch)) return 1;
@@ -731,7 +795,6 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     }
     const int D = ctx->D, Hd = ctx->Hd, T = ctx->T, R = max_batch, Dq = ctx->Dq;
     const size_t M = (size_t)R * T;
-    const int Rpad = R < 128 ? 128 : R;
     if (dev_alloc(ctx, &ctx->x_tok, M * D)) return 1;
     // xn (with its row scales for e4m3) and the tensor maps of the LayerNorm-fed GEMMs' operands
     if (with_ln_operand(ctx, [&](auto op) {
@@ -748,22 +811,15 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
     if (dev_alloc(ctx, &ctx->qkv, M * 3 * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->attn, M * Dq)) return 1;
     if (dev_alloc(ctx, &ctx->hmid, M * Hd)) return 1;
-    if (dev_alloc(ctx, &ctx->mod, (size_t)R * ctx->Nmod)) return 1;
-    if (dev_alloc(ctx, &ctx->c_silu, (size_t)Rpad * D)) return 1;
-    if (dev_alloc(ctx, &ctx->tfreq, (size_t)R * 256)) return 1;
-    if (dev_alloc(ctx, &ctx->h1, (size_t)R * D)) return 1;
     if (dev_alloc(ctx, &ctx->v_net, (size_t)R * ctx->out_chw)) return 1;
     if (alloc_solver_state(ctx, R)) return 1;
 
     bool ok = make_tmap_bf16(&ctx->tm_attn, ctx->attn, M, Dq, kGemmBoxRows);
     ok &= make_tmap_bf16(&ctx->tm_hmid, ctx->hmid, M, Hd, kGemmBoxRows);
-    ok &= make_tmap_bf16(&ctx->tm_csilu, ctx->c_silu, Rpad, D, kGemmBoxRows);
-    ok &= make_tmap_bf16(&ctx->tm_wmod, ctx->w_mod, ctx->Nmod, D, kGemmBoxRows);
     ok &= attn_plan(&ctx->attn_op, ctx->qkv, ctx->attn, T, ctx->dhp, ctx->dh, ctx->H, network_qkv_layout(T, ctx->dhp), R);
     ok &= make_tmap_out(&ctx->tmo_qkv, ctx->qkv, M, 3 * Dq, 3 * Dq, false);
     ok &= make_tmap_out(&ctx->tmo_hmid, ctx->hmid, M, Hd, Hd, false);
     ok &= make_tmap_out(&ctx->tmo_x_tok, ctx->x_tok, M, D, D, true);
-    ok &= make_tmap_out(&ctx->tmo_mod, ctx->mod, R, ctx->Nmod, ctx->Nmod, true);
     for (auto& b : ctx->blk) {
         ok &= make_tmap_bf16(&b.tm_proj, b.w_proj, D, Dq, kGemmBoxRows);
         ok &= make_tmap_bf16(&b.tm_fc2, b.w_fc2, D, Hd, kGemmBoxRows);
@@ -791,24 +847,36 @@ extern "C" int lfm_finalize(lfm_ctx* ctx, int max_batch) {
 
 static int check_ready(lfm_ctx* ctx, int rows, const char* who);
 
-#include "unet_host.inc"
-#include "vae_host.inc"
-
-// The DiT's conditioning for `rows` rows (models/DiT.py:125,264): tf = timestep features of t (t_numel 1 broadcasts),
-// h1 = SiLU(mlp.0(tf)) (fp32), c = SiLU(mlp.2(h1) + table[y]) (bf16, the adaLN GEMM's operand).  y NULL reads the null row
-// table_rows - 1.  w0 [D, 256], w2 [D, D]: D a multiple of 128 up to kConditionMaxD.
-constexpr int kConditionMaxD = 9 * 128;  // skinny_linear_kernel holds a weight row in 9 float4 per lane (its MAXV)
-static int launch_dit_condition(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const long long* y, int rows, int D,
-                                const float* w0, const float* b0, const float* w2, const float* b2, const float* table,
-                                int table_rows, float* tf, float* h1, __nv_bfloat16* c) {
-    timestep_features_kernel<<<rows, 256, 0, s>>>(t, t_numel, tf, rows);
-    LAUNCH_OK();
-    skinny_linear_kernel<0><<<(D + 7) / 8, 256, 0, s>>>(w0, b0, tf, rows, D, 256, nullptr, nullptr, 0, h1, nullptr);
-    LAUNCH_OK();
-    skinny_linear_kernel<1><<<(D + 7) / 8, 256, 0, s>>>(w2, b2, h1, rows, D, D, table, y, table_rows - 1, nullptr, c);
-    LAUNCH_OK();
+// The conditioning stage's kernels for `rows` rows (t_numel 1 broadcasts): tf [rows, feat], h1 = SiLU(w0 tf + b0) [rows, E] and
+// c = SiLU(w2 h1 + b2 + table[row]) [rows, E] (bf16) with condition_mlp_kernel's label rule.  feat and E: condition_k_ok.
+static int launch_condition(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const long long* y, int rows, int feat, int E,
+                            const float* w0, const float* b0, const float* w2, const float* b2, const float* table, int max_row,
+                            int null_row, float* tf, float* h1, __nv_bfloat16* c) {
+    LAUNCH_K(timestep_features_kernel, dim3(rows), 256, 0, s, t, t_numel, tf, feat);
+    LAUNCH_K(condition_mlp_kernel<float>, dim3((E + 7) / 8), 256, 0, s, w0, b0, tf, rows, E, feat, nullptr, nullptr, 0, -1, h1);
+    LAUNCH_K(condition_mlp_kernel<__nv_bfloat16>, dim3((E + 7) / 8), 256, 0, s, w2, b2, h1, rows, E, E, table, y, max_row, null_row, c);
     return 0;
 }
+
+// The conditioning stage for `rows` network rows, then every layer's modulation rows in one GEMM: mod = c W_mod^T + b_mod.  A 0-d t
+// without labels (every unconditional preset) gives the same c for every row: one row is computed and all samples read it.
+// *mod_stride: the stride between samples in mod for the reads of the modulation (n_mod, or 0 for that one row).
+static int cond_launch(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_numel, const long long* y, int rows, int* mod_stride) {
+    const Conditioning& c = ctx->cond;
+    const bool uniform = t_numel == 1 && y == nullptr;
+    const int crows = uniform ? 1 : rows;
+    *mod_stride = uniform ? 0 : c.n_mod;
+    if (launch_condition(ctx, s, t, t_numel, y, crows, c.feat, c.E, c.w0, c.b0, c.w2, c.b2, c.table, c.max_row, c.null_row, c.tf, c.h1,
+                         c.c_silu))
+        return 1;
+    GemmEpi ep{c.b_mod, c.mod, c.n_mod, nullptr, 0, 1};
+    ep.out_map = &c.tmo_mod;
+    COUNT_LAUNCH(launch_gemm(s, c.tm_csilu, c.tm_wmod, crows, c.n_mod, c.E, EPI_BIAS_F32, 0, ep));
+    return 0;
+}
+
+#include "unet_host.inc"
+#include "vae_host.inc"
 
 // Patch embed of M token rows (T = G^2 per sample; row b reads latent b % x_rows): the specialised kernel for p = 2 (C = 4),
 // the generic one, with its 8 patch vectors in dynamic shared memory, for p = 4 and 8.
@@ -847,19 +915,9 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     if (ctx->net != NetKind::DIT) return launch_unet(ctx, s, t, t_numel, x, x_rows, y, rows, x_whole);
     const int D = ctx->D, L = ctx->L, Hd = ctx->Hd, T = ctx->T, Dq = ctx->Dq;
     const int M = rows * T;
-    // Conditioning c = t_emb(t) + y_emb(y) and the adaLN tables.  A 0-d t with y = None (every unconditional
-    // preset) gives the same c for every row: compute ONE row and let all samples read it (table stride 0).
-    const bool uniform_c = (t_numel == 1 && y == nullptr);
-    const int crows = uniform_c ? 1 : rows;
-    const int Nmod = uniform_c ? 0 : ctx->Nmod;  // stride between samples in the modulation table
-    if (launch_dit_condition(ctx, s, t, t_numel, y, crows, D, ctx->t_w0, ctx->t_b0, ctx->t_w2, ctx->t_b2, ctx->ytable,
-                             ctx->d.table_rows, ctx->tfreq, ctx->h1, ctx->c_silu))
-        return 1;
-    {   // all adaLN modulation vectors of the network in one GEMM: mod[crows, (6L+2) D]
-        GemmEpi ep{ctx->b_mod, ctx->mod, ctx->Nmod, nullptr, 0, 1};
-        ep.out_map = &ctx->tmo_mod;
-        COUNT_LAUNCH(launch_gemm(s, ctx->tm_csilu, ctx->tm_wmod, crows, ctx->Nmod, D, EPI_BIAS_F32, 0, ep));
-    }
+    // c = t_emb(t) + y_emb(y) and every adaLN modulation vector of the network: mod [rows or 1, (6L+2) D]
+    int Nmod = 0;  // stride between samples in the modulation table
+    if (cond_launch(ctx, s, t, t_numel, y, rows, &Nmod)) return 1;
     const int ps = ctx->d.patch_size;
     if (launch_patch_embed(ctx, s, x, x_rows, ctx->pe_w, ctx->pe_b, ctx->pos, ctx->x_tok, D, ctx->G, ctx->C, ps, M)) return 1;
     // L2 zig-zag: consecutive kernels sweep the token rows in opposite directions, so each starts on the rows its
@@ -885,7 +943,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
     };
     for (int l = 0; l < L; ++l) {
         BlockW& b = ctx->blk[l];
-        const float* mb = ctx->mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
+        const float* mb = ctx->cond.mod + (size_t)l * 6 * D;  // shift_msa | scale_msa | gate_msa | shift_mlp | scale_mlp | gate_mlp
         {
             GemmEpi ep{b.b_qkv, ctx->qkv, 3 * Dq, nullptr, 0, T};
             ep.out_map = &ctx->tmo_qkv;
@@ -913,7 +971,7 @@ static int launch_network(lfm_ctx* ctx, cudaStream_t s, const float* t, int t_nu
             COUNT_LAUNCH(launch_gemm(s, ctx->tm_hmid, b.tm_fc2, M, D, Hd, EPI_GATE_RESID_F32, 0, ep));
         }
     }
-    const float* mf = ctx->mod + (size_t)6 * L * D;  // shift | scale
+    const float* mf = ctx->cond.mod + (size_t)6 * L * D;  // shift | scale
     return launch_final_layer(ctx, s, ctx->x_tok, mf, mf + D, Nmod, ctx->fin_w, ctx->fin_b, ctx->v_net, M, D, ctx->G, ctx->C, ps);
 }
 
@@ -1605,21 +1663,22 @@ extern "C" int lfm_dbg_quantize_rows_fp8(const float* w, void* codes_e4m3, float
     });
 }
 
-extern "C" int lfm_dbg_dit_condition(const float* t, int t_numel, const long long* y, int rows, int D, const float* w0, const float* b0,
-                                     const float* w2, const float* b2, const float* table, int table_rows, float* tf_out, float* h1_out,
-                                     void* c_bf16, void* stream) {
-    if (rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: rows must be >= 1 (got %d)", rows);
+extern "C" int lfm_dbg_condition(const float* t, int t_numel, const long long* y, int rows, int feat, int E, const float* w0,
+                                 const float* b0, const float* w2, const float* b2, const float* table, int max_row, int null_row,
+                                 float* tf_out, float* h1_out, void* c_bf16, void* stream) {
+    if (rows < 1) return fail(nullptr, "lfm_dbg_condition: rows must be >= 1 (got %d)", rows);
     if (t_numel != 1 && t_numel != rows)
-        return fail(nullptr, "lfm_dbg_dit_condition: t_numel must be 1 or rows (got %d, rows %d)", t_numel, rows);
-    if (D < 128 || D % 128 != 0 || D > kConditionMaxD)
-        return fail(nullptr, "lfm_dbg_dit_condition: D must be a multiple of 128 up to %d (got %d)", kConditionMaxD, D);
-    if (table_rows < 1) return fail(nullptr, "lfm_dbg_dit_condition: table_rows must be >= 1 (got %d)", table_rows);
-    if (t == nullptr || w0 == nullptr || b0 == nullptr || w2 == nullptr || b2 == nullptr || table == nullptr || tf_out == nullptr ||
-        h1_out == nullptr || c_bf16 == nullptr)
-        return fail(nullptr, "lfm_dbg_dit_condition: only y may be NULL");
+        return fail(nullptr, "lfm_dbg_condition: t_numel must be 1 or rows (got %d, rows %d)", t_numel, rows);
+    if (!condition_k_ok(feat) || !condition_k_ok(E))
+        return fail(nullptr, "lfm_dbg_condition: feat and E must be multiples of 128 up to %d (got feat %d, E %d)", kConditionMaxK, feat, E);
+    if (max_row < 0 || null_row < -1 || null_row > max_row)
+        return fail(nullptr, "lfm_dbg_condition: max_row must be >= 0 and null_row in [-1, max_row] (got %d, %d)", max_row, null_row);
+    if (t == nullptr || w0 == nullptr || b0 == nullptr || w2 == nullptr || b2 == nullptr || tf_out == nullptr || h1_out == nullptr ||
+        c_bf16 == nullptr || (table == nullptr && (y != nullptr || null_row >= 0)))
+        return fail(nullptr, "lfm_dbg_condition: only y may be NULL, and table when neither y nor null_row reads it");
     return dbg_run([&](lfm_ctx* ctx) {
-        return launch_dit_condition(ctx, static_cast<cudaStream_t>(stream), t, t_numel, y, rows, D, w0, b0, w2, b2, table, table_rows,
-                                    tf_out, h1_out, static_cast<__nv_bfloat16*>(c_bf16));
+        return launch_condition(ctx, static_cast<cudaStream_t>(stream), t, t_numel, y, rows, feat, E, w0, b0, w2, b2, table, max_row,
+                                null_row, tf_out, h1_out, static_cast<__nv_bfloat16*>(c_bf16));
     });
 }
 
@@ -1861,9 +1920,8 @@ extern "C" int lfm_dbg_groupnorm(const float* a, int Ca, const float* b, int Cb,
         UNetState u;
         u.gn_eps = eps;
         u.max_chunks = max_chunks;
-        push_gn(&u, Src2{a, b, Ca, Cb}, HW, C, gamma, beta, film != nullptr ? 0 : -1, act, static_cast<__nv_bfloat16*>(out_bf16),
-                copy_out, static_cast<__nv_bfloat16*>(raw_out));
-        u.film = const_cast<float*>(film);
+        push_gn(&u, Src2{a, b, Ca, Cb}, HW, C, gamma, beta, film, act, static_cast<__nv_bfloat16*>(out_bf16), copy_out,
+                static_cast<__nv_bfloat16*>(raw_out));
         UOp& st = u.prog[0];
         UOp& ap = u.prog[1];
         ap.gn_src_bf16 = static_cast<const __nv_bfloat16*>(src_bf16);

@@ -385,49 +385,6 @@ conv_in_strip_kernel(ConvInSrc a, ConvInSrc b, int x_rows, const float* __restri
     }
 }
 
-// out.2: conv3x3(C -> 4), pad 1, on the GN+SiLU'd bf16 NHWC operand -> NCHW fp32 velocity (unet.py:591-595).
-// One warp per output pixel, lane = 8-channel slice; weights [4][9][C] fp32 in shared memory.
-__global__ void __launch_bounds__(256)
-conv_out_kernel(const __nv_bfloat16* __restrict__ a, const float* __restrict__ Wr /*[4][9][C]*/,
-                const float* __restrict__ bias, float* __restrict__ v_out, int B, int H, int W, int C) {
-    extern __shared__ float s_w[];
-    for (int i = threadIdx.x; i < 36 * C; i += blockDim.x) s_w[i] = Wr[i];
-    __syncthreads();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total = B * H * W;
-    for (int pix = blockIdx.x * 8 + warp; pix < total; pix += gridDim.x * 8) {
-        const int b = pix / (H * W), h = (pix / W) % H, w = pix % W;
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int tap = 0; tap < 9; ++tap) {
-            const int hh = h + tap / 3 - 1, ww = w + tap % 3 - 1;
-            if (hh < 0 || hh >= H || ww < 0 || ww >= W) continue;  // warp-uniform
-            const __nv_bfloat16* ap = a + (static_cast<size_t>(b) * H * W + static_cast<size_t>(hh) * W + ww) * C;
-            for (int c0 = lane * 8; c0 < C; c0 += 256) {
-                const uint4 u = *reinterpret_cast<const uint4*>(ap + c0);
-                const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&u);
-                float f[8];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const float2 t = __bfloat1622float2(h2[k]);
-                    f[2 * k] = t.x, f[2 * k + 1] = t.y;
-                }
-#pragma unroll
-                for (int o = 0; o < 4; ++o) {
-                    const float* wp = s_w + (o * 9 + tap) * C + c0;
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) acc[o] = fmaf(f[k], wp[k], acc[o]);
-                }
-            }
-        }
-#pragma unroll
-        for (int o = 0; o < 4; ++o) acc[o] = warp_sum(acc[o]);
-        if (lane < 4) {
-            const float r = lane == 0 ? acc[0] : (lane == 1 ? acc[1] : (lane == 2 ? acc[2] : acc[3]));
-            v_out[((static_cast<size_t>(b) * 4 + lane) * H + h) * W + w] = r + bias[lane];
-        }
-    }
-}
-
 // out.2 on the tensor cores: the GEMM writes [B*H*W, 4] (NHWC); this scatters it to the NCHW velocity.
 __global__ void nhwc4_to_nchw_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int HW) {
     pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
@@ -829,60 +786,6 @@ __global__ void conv_weight_repack_kernel(const float* __restrict__ w, __nv_bflo
     const int tap = static_cast<int>((i / Cin) % taps);
     const int o = static_cast<int>(i / (static_cast<size_t>(Cin) * taps));
     out[i] = __float2bfloat16(w[(static_cast<size_t>(o) * Cin + c) * taps + tap]);
-}
-// sinusoidal timestep features of arbitrary even width (nn.py:103-121; cos first, raw t)
-__global__ void timestep_features_dim_kernel(const float* __restrict__ t, int t_numel, float* __restrict__ tf, int B, int dim) {
-    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
-    pdl_trigger();
-    const int b = blockIdx.x;
-    const int half = dim / 2;
-    for (int i = threadIdx.x; i < dim; i += blockDim.x) {
-        const float tv = t[t_numel == 1 ? 0 : b];
-        const int k = i < half ? i : i - half;
-        const float freq = expf(-9.210340371976184f * static_cast<float>(k) / static_cast<float>(half));
-        const float a = tv * freq;
-        tf[static_cast<size_t>(b) * dim + i] = (i < half) ? cosf(a) : sinf(a);
-    }
-}
-
-// general skinny linear (any K % 4 == 0): out[b, j] = act(bias[j] + W[j,:] . in[b,:] (+ table[idx[b], j]))
-// mode 0: SiLU -> fp32;  mode 1: (+table) then SiLU -> bf16
-__global__ void __launch_bounds__(256)
-skinny_linear_gen_kernel(const float* __restrict__ W, const float* __restrict__ bias, const float* __restrict__ in, int B,
-                         int N, int K, const float* __restrict__ table, const long long* __restrict__ idx, int mode,
-                         float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int max_row) {
-    pdl_wait();  // PDL: nothing of the previous kernel's output is touched above this line
-    pdl_trigger();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int j = blockIdx.x * 8 + warp;
-    if (j >= N) return;
-    const float4* wp = reinterpret_cast<const float4*>(W + static_cast<size_t>(j) * K);
-    const float bj = bias[j];
-    for (int b = 0; b < B; ++b) {
-        const float4* ip = reinterpret_cast<const float4*>(in + static_cast<size_t>(b) * K);
-        float acc = 0.f;
-        for (int m = lane; m < K / 4; m += 32) {
-            const float4 w4 = __ldg(wp + m), x4 = __ldg(ip + m);
-            acc = fmaf(w4.x, x4.x, acc);
-            acc = fmaf(w4.y, x4.y, acc);
-            acc = fmaf(w4.z, x4.z, acc);
-            acc = fmaf(w4.w, x4.w, acc);
-        }
-        acc = warp_sum(acc);
-        if (lane == 0) {
-            float v = acc + bj;
-            if (mode == 1 && table != nullptr && idx != nullptr) {
-                long long row = idx[b];
-                row = row < 0 ? 0 : (row > max_row ? max_row : row);  // never read outside the table
-                v += table[static_cast<size_t>(row) * N + j];
-            }
-            v = silu(v);
-            if (mode == 0)
-                out_f32[static_cast<size_t>(b) * N + j] = v;
-            else
-                out_bf16[static_cast<size_t>(b) * N + j] = __float2bfloat16(v);
-        }
-    }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
 """Record tests/golden/dit_fingerprint.npz: fingerprints of the DiT forward (lfm_forward) on the mini_uncond, mini_cond and
-mini_xl2 fixtures and of a 4-step Euler run with CFG on mini_cond, each in the bf16 and the FP8 mode, on cuda:0.
+mini_xl2 fixtures, of the uniform-row forward (0-d t, no labels) and a 4-step Euler run without labels on mini_uncond, and of
+a 4-step Euler run with CFG on mini_cond, each in the bf16 and the FP8 mode, on cuda:0.
 
     python scripts/make_dit_golden.py [OUT.npz]
 
@@ -43,7 +44,8 @@ def _net(g, cfg, fp8, dev):
 
 
 def outputs(dev):
-    """name -> fp32 CPU tensor: per mode, one forward on each fixture ([B] t, labels) and Euler-4 with CFG 1.5 on mini_cond."""
+    """name -> fp32 CPU tensor: per mode, one forward on each fixture ([B] t, labels), the uniform-row forward and Euler-4
+    without labels on mini_uncond, and Euler-4 with CFG 1.5 on mini_cond."""
     res = {}
     for mode in ("bf16", "fp8"):
         for name in FIXTURES:
@@ -51,6 +53,13 @@ def outputs(dev):
             net = _net(g, cfg, mode == "fp8", dev)
             t, x, y = (torch.from_numpy(np.asarray(g[k])).to(dev) for k in ("t_vec", "x", "y"))
             res[f"{mode}_{name}_forward"] = net(t, x, y).cpu()
+            if name == "mini_uncond":
+                # a 0-d t without labels: one conditioning row, read by every sample with stride 0
+                res[f"{mode}_{name}_forward_uniform"] = net(torch.tensor(float(g["t_scalar"]), device=dev), x).cpu()
+                out = lfm_b200.karras_sample(net, x, 5, clip_denoised=False, model_kwargs={}, sigma_min=1e-5, sigma_max=1.0,
+                                             sampler="euler")
+                assert net.last_stats["nfe"] == 4
+                res[f"{mode}_{name}_euler4"] = out.cpu()
             if name == "mini_cond":
                 mk = dict(y=torch.from_numpy(np.asarray(g["y_cfg"])).to(dev), cfg_scale=1.5)
                 out = lfm_b200.karras_sample(net, torch.cat([x, x]), 5, clip_denoised=False, model_kwargs=mk, sigma_min=1e-5,

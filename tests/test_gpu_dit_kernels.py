@@ -14,8 +14,8 @@ Bounds, from the compute types (u = 2^-24 is the fp32 unit roundoff; NV = D / 12
   * FinalLayer (fp32): the same LayerNorm without the bf16 rounding, then a D-term fp32 dot product (D / 32 fmas per lane and a
     5-step butterfly, 16 outputs at p = 2, 32 per chunk otherwise): (D / 32 + 8) u (|W| |y| + |b|) + |W| e_y.  A swapped p / q or c
     index moves a pixel by a whole independent output.  Measured: at most 0.013 of this bound.
-  * conditioning: the timestep features t f_k with f_k = exp(-ln(1e4) k / 128) evaluated in fp32 (the exponent's two roundings,
-    expf's 2 ulp and the product: 24 u |t f_k|; cosf / sinf 1 ulp): (32 |t f_k| + 4) u.  Each skinny linear stage is checked from the
+  * conditioning: the timestep features t f_k with f_k = exp(-ln(1e4) k / half) evaluated in fp32 (the exponent's two roundings,
+    expf's 2 ulp and the product: 24 u |t f_k|; cosf / sinf 1 ulp): (32 |t f_k| + 4) u.  Each MLP layer is checked from the
     kernel's own fp32 input: K / 32 fmas per lane, a 5-step butterfly, the bias and the label row, (K / 32 + 8) u (|W| |in| + |b|
     + |table|), through SiLU (slope <= 1.1); SiLU's __expf is ex2.approx of a rounded product (2^-21 + u |v| relative) and its
     division is IEEE: |silu(v)| (2^-21 + 2^-23 (|v| + 2)).  c is rounded to bf16: one ulp more.  Measured: tf 0.12, h1 0.057, c 0.50.
@@ -151,42 +151,54 @@ def silu_bound(v):
     return v.abs() * torch.sigmoid(v) * (2.0 ** -21 + 2.0 ** -23 * (v.abs() + 2))
 
 
+# Label rules (lfm_dbg_condition's max_row / null_row) of the three networks, for a table of n labels: the DiT's null class is its
+# last row, which y NULL reads; ADM reads label rows only; EDM's map_label table has one all-zero row after its labels (max_row = n).
+LABEL_RULES = {"dit": lambda n: (n - 1, n - 1), "adm": lambda n: (n - 1, -1), "edm": lambda n: (n, -1)}
+CONDITION_CASES = [("dit", 256, 384), ("dit", 256, 1152),     # DiT-S / XL widths
+                   ("adm", 128, 512), ("adm", 256, 1024),     # UNet model_channels 128 / 256: E = 4 model_channels
+                   ("edm", 128, 512), ("edm", 256, 1024),
+                   ("adm", 512, 2048), ("edm", 1024, 4096)]   # K > 1152: weights beyond the registers stream from memory
+
+
 @pytest.mark.parametrize("per_row_t", [False, True])
-@pytest.mark.parametrize("labels", [False, True])   # y NULL (every row reads the null row) / labels that include the null class
+@pytest.mark.parametrize("labels", [False, True])   # y NULL / labels that include the last table row
 @pytest.mark.parametrize("rows", [1, 7, 256])       # 256: CFG doubling of max_batch 128
-@pytest.mark.parametrize("D", [384, 1152])          # 1152: the 9-float4 limit of skinny_linear_kernel
-def test_dit_condition(dev, D, rows, labels, per_row_t):
-    g = gen(D + rows + 2 * labels + per_row_t)
+@pytest.mark.parametrize("net,feat,E", CONDITION_CASES)
+def test_condition(dev, net, feat, E, rows, labels, per_row_t):
+    g = gen(E + rows + 2 * labels + per_row_t)
     t_numel = rows if per_row_t else 1
     t = torch.rand(t_numel, device="cuda", generator=g)
-    table_rows = NULL_CLASS + 1
+    max_row, null_row = LABEL_RULES[net](NULL_CLASS)
     y = None
     if labels:
-        y = torch.randint(0, NULL_CLASS, (rows,), device="cuda", generator=g)
-        y[::3] = NULL_CLASS
-    w0, b0 = randn(D, 256, g=g) * (2 / 16), randn(D, g=g) * 0.5
-    w2, b2 = randn(D, D, g=g) * (2 / math.sqrt(D)), randn(D, g=g) * 0.5
-    table = randn(table_rows, D, g=g)
-    tf, h1, c = nan_like((rows, 256)), nan_like((rows, D)), nan_like((rows, D), torch.bfloat16)
-    done(_lib.load().lfm_dbg_dit_condition(ptr(t), t_numel, tk.P(y), rows, D, ptr(w0), ptr(b0), ptr(w2), ptr(b2), ptr(table),
-                                           table_rows, ptr(tf), ptr(h1), ptr(c), None))
-    what = f"D {D} rows {rows} labels {labels} t_numel {t_numel}"
+        y = torch.randint(0, max_row, (rows,), device="cuda", generator=g)
+        y[::3] = max_row
+    w0, b0 = randn(E, feat, g=g) * (2 / math.sqrt(feat)), randn(E, g=g) * 0.5
+    w2, b2 = randn(E, E, g=g) * (2 / math.sqrt(E)), randn(E, g=g) * 0.5
+    table = randn(max_row + 1, E, g=g)
+    tf, h1, c = nan_like((rows, feat)), nan_like((rows, E)), nan_like((rows, E), torch.bfloat16)
+    done(_lib.load().lfm_dbg_condition(ptr(t), t_numel, tk.P(y), rows, feat, E, ptr(w0), ptr(b0), ptr(w2), ptr(b2), ptr(table),
+                                       max_row, null_row, ptr(tf), ptr(h1), ptr(c), None))
+    what = f"{net} {feat} -> {E} rows {rows} labels {labels} t_numel {t_numel}"
     # timestep features [cos | sin](t f_k)
-    k = torch.arange(128, device="cuda", dtype=torch.float64)
-    a = t.double().expand(rows)[:, None] * torch.exp(-math.log(1e4) * k / 128)
+    half = feat // 2
+    k = torch.arange(half, device="cuda", dtype=torch.float64)
+    a = t.double().expand(rows)[:, None] * torch.exp(-math.log(1e4) * k / half)
     a = torch.cat([a, a], 1)
-    tf_ref = torch.cat([torch.cos(a[:, :128]), torch.sin(a[:, 128:])], 1)
+    tf_ref = torch.cat([torch.cos(a[:, :half]), torch.sin(a[:, half:])], 1)
     tk.assert_within(tf, tf_ref, U * (32 * a.abs() + 4), f"condition tf: {what}")
     # h1 = SiLU(w0 tf + b0), from the kernel's tf
     v = tf.double() @ w0.double().t() + b0.double()
     va = tf.double().abs() @ w0.double().abs().t() + b0.double().abs()
-    tk.assert_within(h1, v * torch.sigmoid(v), 1.1 * (256 / 32 + 8) * U * va + silu_bound(v), f"condition h1: {what}")
-    # c = bf16(SiLU(w2 h1 + b2 + table[y])), from the kernel's h1
-    row = y if y is not None else torch.full((rows,), table_rows - 1, device="cuda")
-    v = h1.double() @ w2.double().t() + b2.double() + table.double()[row]
-    va = h1.double().abs() @ w2.double().abs().t() + b2.double().abs() + table.double()[row].abs()
+    tk.assert_within(h1, v * torch.sigmoid(v), 1.1 * (feat / 32 + 8) * U * va + silu_bound(v), f"condition h1: {what}")
+    # c = bf16(SiLU(w2 h1 + b2 + table[row])), from the kernel's h1
+    v = h1.double() @ w2.double().t() + b2.double()
+    va = h1.double().abs() @ w2.double().abs().t() + b2.double().abs()
+    if y is not None or null_row >= 0:
+        row = y if y is not None else torch.full((rows,), null_row, device="cuda")
+        v, va = v + table.double()[row], va + table.double()[row].abs()
     ref = v * torch.sigmoid(v)
-    tk.assert_within(c, ref, tk.bf16_ulp(ref) + 1.1 * (D / 32 + 8) * U * va + silu_bound(v), f"condition c: {what}")
+    tk.assert_within(c, ref, tk.bf16_ulp(ref) + 1.1 * (E / 32 + 8) * U * va + silu_bound(v), f"condition c: {what}")
 
 
 # ------------------------------------------------------------------------------------------------ patch embed

@@ -202,14 +202,16 @@ def load_recipe():
     return mod
 
 
-def test_unconditioned_unet_bit_identical_to_the_recorded_fingerprint(dev):
-    """A 4-channel UNetModel forward and a celeb512 dopri5 trajectory give the bytes recorded before conv_in took concatenated
-    conditions (tests/golden/unet_fingerprint.npz, scripts/make_unet_golden.py)."""
+def test_unet_and_edm_bit_identical_to_the_recorded_fingerprint(dev):
+    """The UNetModel forwards (4-channel, class-conditional) and a celeb512 dopri5 trajectory, and the DhariwalUNet forwards (without
+    and with labels, forward_with_cfg) and a CFG Euler run, give the bytes recorded by scripts/make_unet_golden.py
+    (tests/golden/unet_fingerprint.npz)."""
     g = np.load(os.path.join(ROOT, "tests", "golden", "unet_fingerprint.npz"))
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     if int(g["num_sms"]) != sms:
         pytest.skip(f"fingerprint recorded with {int(g['num_sms'])} SMs ({g['device']}); the split-K plan differs on {sms}")
     got = load_recipe().fingerprint(dev)
+    assert sorted(got) == sorted(k for k in g.files if k.endswith(("_sha256", "_sub")))
     for k, v in got.items():
         if k.endswith("_sub"):
             assert np.array_equal(v, g[k]), k

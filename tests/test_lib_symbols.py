@@ -132,14 +132,6 @@ def test_kernel_entries_refuse_bad_arguments(lib):
     refused(ln(None, None, None, None, 6, 256, 512, 1024, 0, None), "mod_stride")
     refused(ln(None, None, None, None, 0, 256, 512, 1024, 2, None), "down")
     refused(ln(None, None, None, None, 0, 256, 512, 1024, 0, None), "NULL")
-    # lfm_dbg_dit_condition(t, t_numel, y, rows, D, w0, b0, w2, b2, table, table_rows, tf, h1, c, stream)
-    cond = lib.lfm_dbg_dit_condition
-    refused(cond(None, 1, None, 0, 384, None, None, None, None, None, 11, None, None, None, None), "rows")
-    refused(cond(None, 3, None, 4, 384, None, None, None, None, None, 11, None, None, None, None), "t_numel")
-    refused(cond(None, 1, None, 4, 1280, None, None, None, None, None, 11, None, None, None, None), "D")
-    refused(cond(None, 1, None, 4, 200, None, None, None, None, None, 11, None, None, None, None), "D")
-    refused(cond(None, 1, None, 4, 384, None, None, None, None, None, 0, None, None, None, None), "table_rows")
-    refused(cond(None, 4, None, 4, 384, None, None, None, None, None, 11, None, None, None, None), "NULL")
     # lfm_dbg_patch_embed(x, x_rows, Wt, bias, pos, tok, D, G, C, p, M, stream)
     pe = lib.lfm_dbg_patch_embed
     refused(pe(None, 1, None, None, None, None, 384, 16, 4, 3, 256, None), "p")
@@ -157,6 +149,33 @@ def test_kernel_entries_refuse_bad_arguments(lib):
     refused(fl(None, None, None, 2, None, None, None, 256, 384, 16, 4, 2, None), "mod_stride")
     refused(fl(None, None, None, 0, None, None, None, 0, 384, 16, 4, 2, None), "M")
     refused(fl(None, None, None, 0, None, None, None, 256, 384, 16, 4, 2, None), "NULL")
+
+
+def test_condition_entry_refuses_bad_arguments(lib):
+    """lfm_dbg_condition checks its shapes, its label rule and its pointers before it touches the device, and names the bad
+    argument: the K of both MLP layers (feat and E) is a multiple of 128 up to 4096."""
+    from lfm_b200 import _lib
+
+    def refused(rc, word):
+        assert rc != 0
+        assert word in _lib.last_error(), _lib.last_error()
+
+    d = ctypes.c_void_p(64)   # never dereferenced: each call below is refused before the device is touched
+    # lfm_dbg_condition(t, t_numel, y, rows, feat, E, w0, b0, w2, b2, table, max_row, null_row, tf, h1, c, stream)
+    cond = lib.lfm_dbg_condition
+    refused(cond(d, 1, None, 0, 256, 384, d, d, d, d, d, 10, 10, d, d, d, None), "rows")
+    refused(cond(d, 3, None, 4, 256, 384, d, d, d, d, d, 10, 10, d, d, d, None), "t_numel")
+    refused(cond(d, 1, None, 4, 256, 4224, d, d, d, d, d, 10, 10, d, d, d, None), "E 4224")      # beyond 4096
+    refused(cond(d, 1, None, 4, 256, 200, d, d, d, d, d, 10, 10, d, d, d, None), "E 200")       # not a multiple of 128
+    refused(cond(d, 1, None, 4, 192, 384, d, d, d, d, d, 10, 10, d, d, d, None), "feat 192")
+    refused(cond(d, 1, None, 4, 8192, 1024, d, d, d, d, d, 10, 10, d, d, d, None), "feat 8192")
+    refused(cond(d, 1, None, 4, 256, 384, d, d, d, d, d, -1, -1, d, d, d, None), "max_row must be >= 0 and null_row in [-1, max_row] (got -1, -1)")
+    refused(cond(d, 1, None, 4, 256, 384, d, d, d, d, d, 10, 11, d, d, d, None), "(got 10, 11)")
+    refused(cond(d, 1, None, 4, 256, 384, d, d, d, d, d, 10, -2, d, d, d, None), "(got 10, -2)")
+    refused(cond(d, 4, None, 4, 256, 384, None, d, d, d, d, 10, 10, d, d, d, None), "NULL")
+    refused(cond(d, 4, None, 4, 256, 384, d, d, d, d, d, 10, 10, d, None, d, None), "NULL")
+    refused(cond(d, 4, None, 4, 256, 384, d, d, d, d, None, 10, 10, d, d, d, None), "NULL")   # the null row reads the table
+    refused(cond(d, 4, d, 4, 256, 384, d, d, d, d, None, 10, -1, d, d, d, None), "NULL")      # so do labels
 
 
 def test_attention_entry_refuses_bad_arguments(lib):
