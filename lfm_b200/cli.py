@@ -7,7 +7,8 @@
 Same flags, defaults and modes as the reference (test_flow_latent.py:302-408): default "inference" (one batch ->
 image grid), ``--compute_nfe``, ``--measure_time``, ``--compute_fid`` (generation loop with the reference's file
 indexing; with ``--inception_weights FILE`` the FID itself is computed on the device from the decoded uint8 batches,
-lfm_b200/fid.py, and printed / logged as the reference does, test_flow_latent.py:274-282).  Under
+lfm_b200/fid.py, and printed / logged as the reference does, test_flow_latent.py:274-282; ``--compute_is`` adds the
+Inception Score of the same images, lfm_b200/inception_score.py).  Under
 ``torchrun`` (RANK/WORLD_SIZE set) it behaves like test_flow_latent_ddp.py: one process per GPU, per-rank batches,
 seed = seed + rank, file index j * world + rank + total.
 
@@ -101,6 +102,10 @@ def build_parser():
                    help="local pt_inception-2015-12-05-6726825d.pth: compute the FID on the device in the --compute_fid loop")
     p.add_argument("--synthetic_inception", type=int, default=None, metavar="SEED",
                    help="seeded Inception weights (plumbing check only; the number is meaningless)")
+    p.add_argument("--compute_is", action="store_true", default=False,
+                   help="--compute_fid: also the Inception Score of the generated images, on the device (needs "
+                        "--inception_weights or --synthetic_inception)")
+    p.add_argument("--is_splits", type=int, default=10, help="--compute_is: number of splits of the generated images")
     p.add_argument("--no_save", action="store_true", help="--compute_fid: do not write the JPEG files")
     p.add_argument("--out_dir", type=str, default=".")
     p.add_argument("--measure_reps", type=int, default=300)
@@ -269,6 +274,8 @@ def main(argv=None):
     from . import dist as ldist
     from .random_util import get_generator
 
+    if args.compute_is and not args.compute_fid:
+        raise ValueError("--compute_is scores the --compute_fid generation loop: add --compute_fid")
     rank, world, local = ldist.init_from_env()
     args.world_size = world
     torch.set_grad_enabled(False)
@@ -326,14 +333,25 @@ def main(argv=None):
             torch.distributed.barrier()
         total = 0
         sink = ImageSink(device, args.writer_threads) if vae is not None and not args.no_save else None
-        fid_acc = None
+        fid_acc = is_stats = None
+        if args.compute_is and args.inception_weights is None and args.synthetic_inception is None:
+            raise ValueError("--compute_is needs the Inception weights: --inception_weights FILE or --synthetic_inception SEED")
         if args.inception_weights is not None or args.synthetic_inception is not None:
             if vae is None:
                 raise ValueError("the FID needs decoded images: drop --no_decode")
             from . import fid as lfid
-            net = (lfid.FIDInception.from_file(args.inception_weights) if args.inception_weights is not None
-                   else lfid.FIDInception(lfid.synthetic_inception_state_dict(args.synthetic_inception)))
+            logits = args.compute_is
+            if args.inception_weights is not None:
+                net = lfid.FIDInception.from_file(args.inception_weights, with_logits=logits)
+            else:
+                sd = lfid.synthetic_inception_state_dict(args.synthetic_inception)
+                if logits:
+                    sd.update(lfid.synthetic_fc_state_dict(args.synthetic_inception))
+                net = lfid.FIDInception(sd, with_logits=logits)
             fid_acc = lfid.FIDAccumulator(net, device)
+            if args.compute_is:
+                from . import inception_score as lis
+                is_stats = lis.ISStatistics(args.is_splits, total_samples, device)
         for i in range(iters):
             out = run_sampling(n, generator, as_uint8=True)
             if vae is None:
@@ -344,6 +362,8 @@ def main(argv=None):
                     out = (torch.clamp((out + 1.0) / 2.0, 0, 1) * 255.0).permute(0, 2, 3, 1).to(torch.uint8)
                 if fid_acc is not None:
                     fid_acc.update(out)           # features + running statistics on the device; no file round trip
+                if is_stats is not None:          # image j of this batch is file index j * world + rank + total
+                    is_stats.update(lis.inception_probs(fid_acc.net, out, fid_acc.batch), rank + total, world)
                 if sink is not None:
                     sink.put(out, ["{}/{}.jpg".format(save_dir, ldist.file_index(j, world, rank, total))
                                    for j in range(out.shape[0])])
@@ -361,6 +381,14 @@ def main(argv=None):
                 if args.output_log:
                     with open(args.output_log, "a") as f:
                         f.write("Epoch = {}, FID = {}\n".format(args.epoch_id, value))
+            if is_stats is not None:
+                is_stats.all_reduce()                             # one all-reduce of the [S, 1002] split sums
+                is_mean, is_std = is_stats.finalize()
+                if rank == 0:
+                    print("IS = {} +/- {}".format(is_mean, is_std))
+                    if args.output_log:
+                        with open(args.output_log, "a") as f:
+                            f.write("Epoch = {}, IS = {} +/- {}\n".format(args.epoch_id, is_mean, is_std))
         elif rank == 0:
             print("samples written to", save_dir, "- pass --inception_weights FILE for the FID, or run pytorch_fid on them")
         return 0

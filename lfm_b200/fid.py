@@ -135,7 +135,8 @@ def _all_convs():
 
 def inception_state_dict_shapes() -> Dict[str, Tuple[int, ...]]:
     """Key -> shape of the tensors :meth:`FIDInception.load_state_dict_folded` consumes (the torchvision names the
-    published weight file uses; its ``fc.*`` and ``num_batches_tracked`` entries are ignored)."""
+    published weight file uses; its ``num_batches_tracked`` entries are ignored, and its ``fc.*`` entries are read only by
+    a network built ``with_logits``, see :data:`FC_SHAPES`)."""
     out = {}
     for name, (_, _, cin, cout, k, _, _) in _all_convs():
         out[f"{name}.conv.weight"] = (cout, cin, k[0], k[1])
@@ -144,14 +145,21 @@ def inception_state_dict_shapes() -> Dict[str, Tuple[int, ...]]:
     return out
 
 
+FC_SHAPES = {"fc.weight": (1008, 2048), "fc.bias": (1008,)}   # the graph's softmax/logits layer: 1008 classes
+
+
+def _keyed_generator(seed: int, key: str) -> torch.Generator:
+    import zlib
+    return torch.Generator().manual_seed((seed * 1000003 + zlib.crc32(key.encode())) % (2 ** 31))
+
+
 def synthetic_inception_state_dict(seed: int = 1) -> Dict[str, torch.Tensor]:
     """Seeded stand-in for the published weights (there is no network here): He-scaled convolutions and BatchNorm
     statistics near the identity, every tensor drawn from a generator keyed on (seed, crc32(key)) so that the
     reference-side fixture script and the tests build the identical dictionary without shipping 95 MB."""
-    import zlib
     sd = {}
     for key, shape in inception_state_dict_shapes().items():
-        g = torch.Generator().manual_seed((seed * 1000003 + zlib.crc32(key.encode())) % (2 ** 31))
+        g = _keyed_generator(seed, key)
         if key.endswith("conv.weight"):
             fan_in = shape[1] * shape[2] * shape[3]
             t = torch.randn(shape, generator=g) * (2.0 / fan_in) ** 0.5
@@ -163,16 +171,34 @@ def synthetic_inception_state_dict(seed: int = 1) -> Dict[str, torch.Tensor]:
     return sd
 
 
-class FIDInception(torch.nn.Module):
-    """pool3 (2048-d) features of the FID Inception graph; see the module docstring."""
+def synthetic_fc_state_dict(seed: int = 1) -> Dict[str, torch.Tensor]:
+    """Seeded stand-in for the ``fc.*`` classifier of the published file, keyed as :func:`synthetic_inception_state_dict`
+    is: a weight of std ``4 / sqrt(2048)`` (logits of a few units, so the softmax is neither flat nor one-hot on the
+    stand-in trunk's features) and a bias of std 0.05."""
+    sd = {}
+    for key, shape in FC_SHAPES.items():
+        g = _keyed_generator(seed, key)
+        sd[key] = torch.randn(shape, generator=g) * (4.0 / 2048 ** 0.5 if key == "fc.weight" else 0.05)
+    return sd
 
-    def __init__(self, state_dict: Optional[Dict[str, torch.Tensor]] = None, allow_tf32: bool = False):
+
+class FIDInception(torch.nn.Module):
+    """pool3 (2048-d) features of the FID Inception graph; see the module docstring.  With ``with_logits`` it also holds
+    the graph's ``fc`` layer (``fc.weight [1008, 2048]``, ``fc.bias [1008]`` of the same weight file, loaded strictly)
+    and :meth:`logits` gives the 1008 class logits the Inception Score uses (lfm_b200/inception_score.py)."""
+
+    def __init__(self, state_dict: Optional[Dict[str, torch.Tensor]] = None, allow_tf32: bool = False,
+                 with_logits: bool = False):
         super().__init__()
         self.allow_tf32 = bool(allow_tf32)
+        self.with_logits = bool(with_logits)
         self._loaded = False
         for name, (_, _, cin, cout, k, _, _) in _all_convs():
             self.register_buffer(self._w(name), torch.zeros(cout, cin, k[0], k[1]), persistent=False)
             self.register_buffer(self._b(name), torch.zeros(cout), persistent=False)
+        if self.with_logits:
+            self.register_buffer("fc_w", torch.zeros(FC_SHAPES["fc.weight"]), persistent=False)
+            self.register_buffer("fc_b", torch.zeros(FC_SHAPES["fc.bias"]), persistent=False)
         if state_dict is not None:
             self.load_state_dict_folded(state_dict)
 
@@ -195,11 +221,18 @@ class FIDInception(torch.nn.Module):
     @torch.no_grad()
     def load_state_dict_folded(self, sd: Dict[str, torch.Tensor]) -> None:
         """Folds BN(eps 1e-3, eval mode) into each convolution in fp64: w' = w * g / sqrt(var + eps),
-        b' = beta - mean * g / sqrt(var + eps).  Raises KeyError / ValueError on a missing or mis-shaped tensor."""
+        b' = beta - mean * g / sqrt(var + eps).  Raises KeyError / ValueError on a missing or mis-shaped tensor.  The
+        ``fc.*`` entries are read only by a network built ``with_logits``; it raises ValueError when they are missing."""
         shapes = inception_state_dict_shapes()
         missing = [k for k in shapes if k not in sd]
         if missing:
             raise KeyError(f"Inception state dict lacks {len(missing)} tensors, e.g. {missing[:3]}")
+        if self.with_logits:
+            missing = [k for k in FC_SHAPES if k not in sd]
+            if missing:
+                raise ValueError(f"Inception state dict lacks {missing}: the class logits need the graph's fc layer "
+                                 "(pt_inception-2015-12-05-6726825d.pth has it)")
+            shapes = {**shapes, **FC_SHAPES}
         for k, shp in shapes.items():
             if tuple(sd[k].shape) != shp:
                 raise ValueError(f"{k}: shape {tuple(sd[k].shape)}, expected {shp}")
@@ -209,6 +242,9 @@ class FIDInception(torch.nn.Module):
             b = sd[f"{name}.bn.bias"].double() - sd[f"{name}.bn.running_mean"].double() * g
             getattr(self, self._w(name)).copy_((w * g[:, None, None, None]).float())
             getattr(self, self._b(name)).copy_(b.float())
+        if self.with_logits:
+            self.fc_w.copy_(sd["fc.weight"].float())
+            self.fc_b.copy_(sd["fc.bias"].float())
         self._loaded = True
 
     # -- interpreter ---------------------------------------------------------------------------------------------------
@@ -251,9 +287,13 @@ class FIDInception(torch.nn.Module):
 
     @torch.no_grad()
     def forward(self, images: torch.Tensor) -> torch.Tensor:
+        return self.trunk(self.prepare(images))
+
+    @torch.no_grad()
+    def trunk(self, x: torch.Tensor) -> torch.Tensor:
+        """Prepared ``[B, 3, 299, 299]`` input in [-1, 1] -> ``[B, 2048]`` pool3 features."""
         if not self._loaded:
             raise RuntimeError("FIDInception has no weights: load_state_dict_folded / from_file first")
-        x = self.prepare(images)
         cudnn_tf32 = torch.backends.cudnn.allow_tf32
         torch.backends.cudnn.allow_tf32 = self.allow_tf32
         try:
@@ -265,6 +305,19 @@ class FIDInception(torch.nn.Module):
             return x.mean(dim=(2, 3))
         finally:
             torch.backends.cudnn.allow_tf32 = cudnn_tf32
+
+    @torch.no_grad()
+    def logits(self, x: torch.Tensor) -> torch.Tensor:
+        """Prepared ``[B, 3, 299, 299]`` input in [-1, 1] -> ``[B, 1008]`` logits: the trunk, then ``fc`` in fp32
+        (the graph's ``softmax/logits``)."""
+        if not self.with_logits:
+            raise RuntimeError("FIDInception was built without its fc layer: pass with_logits=True")
+        matmul_tf32 = torch.backends.cuda.matmul.allow_tf32
+        torch.backends.cuda.matmul.allow_tf32 = self.allow_tf32
+        try:
+            return F.linear(self.trunk(x), self.fc_w, self.fc_b)
+        finally:
+            torch.backends.cuda.matmul.allow_tf32 = matmul_tf32
 
 
 # ---------------------------------------------------------------------------------------------------------------------
